@@ -26,7 +26,8 @@ const char* ws_last_error(void);
  *      and is the GPU back-end for `SpeakerModel::ExtractEmbedding` (runtime/core/speaker/speaker_model.h:25-32).
  * model_name: ECAPA_TDNN_c512 | ECAPA_TDNN_GLOB_c512 | ECAPA_TDNN_c1024 | ECAPA_TDNN_GLOB_c1024 | ResNet18 |
  *             ResNet34 | CAMPPlus; SURVEY section 8(f) rank 4: ResNet50 | ResNet101 | ResNet152 | ResNet221 | ResNet293 |
- *             XVEC | Res2Net34_Base | Res2Net34_Large | ERes2Net34_Base | ERes2Net34_Large | ERes2Net34_aug.
+ *             XVEC | Res2Net34_Base | Res2Net34_Large | ERes2Net34_Base | ERes2Net34_Large | ERes2Net34_aug |
+ *             SimAM_ResNet34_ASP | SimAM_ResNet100_ASP.
  * precision:  "fp32" (exact IEEE fp32 FFMA path, parity <= 1e-4), "tf32x3" (tensor cores with 3xTF32 error compensation,
  *             fp32-grade accuracy), "tf32", "bf16", "fp16" (wgmma tensor cores). */
 int ws_engine_create(const char* model_name, const char* precision, int feat_dim, int embed_dim, int device,
@@ -150,6 +151,27 @@ typedef struct {
     float* colsum;
 } ws_conv_desc;
 int ws_conv(const ws_conv_desc* d, void* stream);
+
+/* ---- SimAM attention + residual + ReLU of a SimAM-ResNet block (samresnet.py:57-70), exported for parity tests:
+ *      out = relu(y * sigmoid((y - mean)^2 / (4 (var + lambda_p)) + 0.5) + res), mean / var per (b, c) over F x T_b
+ *      (var divides by F*T_b - 1).  Element (b, f, t, c) of res / out is at b*sb + f*sf + t*st + c (elements); res may
+ *      equal out.  All pointers are device pointers. */
+typedef struct {
+    const void* y;            /* [B][F][T][y_ld], channels [0,C), dtype below */
+    long long y_ld;
+    int B, F, T, C;
+    const int* lens;          /* int32[B] frames per utterance (rows t >= lens[b] are ignored and written as zeros) or NULL */
+    float lambda_p;           /* 1e-4 in the reference */
+    const void* res;
+    long long res_sb, res_sf, res_st;
+    void* out;
+    long long out_sb, out_sf, out_st;
+    void* out_lo;             /* dtype 0 only, optional: out - tf32_trunc(out) with out's strides */
+    int dtype;                /* 0 fp32, 1 bf16, 2 fp16 */
+    float* stats;             /* fp32 [B][2][C] (written): mean, variance */
+    float* partial;           /* fp32 scratch [B][F][C][2] */
+} ws_simam_desc;
+int ws_simam(const ws_simam_desc* d, void* stream);
 
 /* ---- two-covariance PLDA scorer: replaces TwoCovPLDA.transform_embedding / log_likelihood_ratio / the trial
  *      loop of eval_sv (wespeaker/utils/plda/two_cov_plda.py:156-184,186-256), fp64 like the reference. */

@@ -1,5 +1,6 @@
 // ASTP tail in one launch: attention logits + softmax over time + weighted mean / std (pooling_layers.py:119-144,
-//   alpha = softmax(linear2(tanh(linear1(x))), dim=T);  mean = sum alpha x;  std = sqrt(clamp(sum alpha x^2 - mean^2, 1e-7))).
+//   alpha = softmax(linear2(tanh(linear1(x))), dim=T);  mean = sum alpha x;  std = sqrt(clamp(sum alpha x^2 - mean^2, var_floor)),
+//   var_floor 1e-7; SimAM-ResNet's ASP, pooling_layers.py:188-204, is the same tail with a ReLU -> BN hidden layer and 1e-5).
 // linear1 (+tanh) stays a conv-GEMM launch that leaves H [B][T][128]; this kernel replaces the linear2 launch (which wrote
 // the [B][T][C] logits, 157 MB at B = 256) and the statistics launch (which read them back together with x):
 //
@@ -222,7 +223,7 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
                         const float mean = s1[h] / s0[h];
                         const float var = s2[h] / s0[h] - mean * mean;
                         p.out[(long long)b * 2 * p.C + c] = mean;
-                        p.out[(long long)b * 2 * p.C + p.C + c] = sqrtf(fmaxf(var, 1e-7f));
+                        p.out[(long long)b * 2 * p.C + p.C + c] = sqrtf(fmaxf(var, p.var_floor));
                     }
                 }
             }

@@ -339,6 +339,7 @@ struct WsAstpParams {
     int grid;
     const int* lens;    // length-masked batch: frames of each utterance, or null
     long long* prof;    // WS_ASTP_PROF: [grid][16] wait-cycle counters per role
+    float var_floor;    // std = sqrt(max(var, var_floor))
 };
 
 // fused Res2 chain (ws_res2_fused.cu)

@@ -42,6 +42,7 @@ bool take_op_trace(std::string* json) {
 }
 static std::string jp(const void* p) { char b[32]; snprintf(b, sizeof b, "%llu", (unsigned long long)p); return b; }
 static std::string jv(const char* name, long long v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%lld", name, v); return b; }
+static std::string jf(float v) { char b[32]; snprintf(b, sizeof b, "%.9g", (double)v); return b; }
 static std::string view_json(const View& v) {
     return "{\"p\":" + jp(v.p) + "," + jv("B", v.B) + "," + jv("F", v.F) + "," + jv("T", v.T) + "," + jv("C", v.C) + "," + jv("ld", v.ld) + "}";
 }
@@ -520,7 +521,8 @@ bool make_res2_op(const View& x, const View& out, const void* W7, const float* b
     return true;
 }
 
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, Op* op, bool* unsupported, const int* lens) {
+bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, Op* op, bool* unsupported,
+                  const int* lens) {
     *unsupported = false;
     if (x.dt == WS_F32 || h.dt != x.dt || x.C % 128 != 0 || h.C != 128 || h.ld != 128 || x.F != 1 || h.F != 1 || h.T != x.T ||
         h.B != x.B || getenv("WS_NO_ASTP_FUSED")) {
@@ -548,6 +550,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, Op
         if (!encode_map(&q->xmap, x.dt, x.p, 3, dims, str, box, 0)) return false;
     }
     q->x = x.p; q->x_ld = x.ld; q->out = stats; q->B = x.B; q->T = x.T; q->C = x.C; q->dtype = x.dt; q->lens = lens;
+    q->var_floor = var_floor;
     // channel blocks per unit: the largest g whose static round-robin over the SMs stays within 8 % of the best balance
     const int nblk = x.C / 128, sms = ws_num_sms();
     double best = 0.0;
@@ -591,7 +594,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, Op
     *op = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
     if (plan_check_mode())
         set_op_trace("{\"kind\":\"astp_fused\",\"es\":2,\"x\":" + view_json(x) + ",\"h\":" + view_json(h) + ",\"W2\":" + jp(W2) + ",\"stats\":" + jp(stats) +
-                     ",\"lens\":" + jp(lens) + "}");
+                     ",\"lens\":" + jp(lens) + ",\"eps\":" + jf(var_floor) + "}");
     {
         char buf[160];
         snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);

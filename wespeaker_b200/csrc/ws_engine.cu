@@ -575,7 +575,7 @@ bool build_ecapa(Builder& b) {
         if (e.use_tc >= 2 && e.opt("astp_fused", 1) && b.good()) {
             Op op;
             bool unsupported = false;
-            if (make_astp_op(frame, hid, W2d, stats, &op, &unsupported, l0)) { b.push(std::move(op)); fused = true; }
+            if (make_astp_op(frame, hid, W2d, stats, 1e-7f, &op, &unsupported, l0)) { b.push(std::move(op)); fused = true; }
             else if (!unsupported) { b.ok = false; return false; }
         }
         if (!fused) {
@@ -585,8 +585,8 @@ bool build_ecapa(Builder& b) {
             b.conv_simple(hid, logits, W2d, 1, 1, 1, 1, 0, 0, 1, 1, ep2);
             View fr = frame, lg = logits;
             set_op_trace("{\"kind\":\"astp_stats\"," + Builder::ti("es", ws_esize(fr.dt)) + "," + Builder::tview("x", fr) + "," + Builder::tview("logits", lg) + "," +
-                         Builder::tp("stats", stats) + "," + Builder::tp("lens", l0) + "}");
-            b.push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, B, T, 1536, fr.ld, stats, s, l0); }, "astp_stats");
+                         Builder::tp("stats", stats) + "," + Builder::tp("lens", l0) + ",\"eps\":1e-07}");
+            b.push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, B, T, 1536, fr.ld, stats, 1e-7f, s, l0); }, "astp_stats");
         }
     }
     {   // bn(3072) then linear (ecapa_tdnn.py:230-231): fold the affine into the linear; optional bn2 (emb_bn)
@@ -971,7 +971,7 @@ static bool aff(Builder& b, const std::string& p, const View& x, const View& y, 
 }
 
 // 3x3 pad-1 conv (+ folded BN shift) -> act over `in` (and, when in2 != nullptr, over in + in2 with the weights repeated):
-// the halo-resident kernel where it applies, else the generic conv-GEMM.  act: WS_ACT_RELU20 or WS_ACT_NONE.
+// the halo-resident kernel where it applies, else the generic conv-GEMM.  act: WS_ACT_RELU20, WS_ACT_RELU or WS_ACT_NONE.
 static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, const View* in2, const View& out, const std::vector<float>& w9,
                          const std::vector<float>& bias, int act, int stride, int lvl) {   // lvl: stride level of `out` (length-masked plans)
     const int Cin = in.C, Cout = out.C;
@@ -982,7 +982,8 @@ static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, cons
         if (b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0 && (stride == 1 || b.e.opt("conv3x3_strided", 1) != 0)) {
             Op op;
             bool unsupported = false;
-            if (make_conv3x3_op(in, out, W, bd, nullptr, act == WS_ACT_RELU20 ? 2 : 0, &op, &unsupported, stride, stride, b.lens(lvl))) {
+            if (make_conv3x3_op(in, out, W, bd, nullptr, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, &op, &unsupported, stride, stride,
+                                b.lens(lvl))) {
                 b.push(std::move(op));
                 return b.good();
             }
@@ -1179,6 +1180,166 @@ bool build_res2net(Builder& b, const Res2Cfg& c) {
     }
     if (!b.good()) return false;
     return resnet_tail(b, cur, E);
+}
+
+// ----------------------------------------------------------------------------------------------- SimAM-ResNet + ASP
+// samresnet.py:21-167 (SimAMBasicBlock; the ResNet trunk under `front.`), pooling_layers.py:151-204 (ASP).  A block is conv1
+// (+bn1, ReLU) and conv2 (+bn2) on res2_conv3x3, the 1x1 strided downsample conv (+BN) written into the block's output
+// buffer, then the SimAM statistics op and the apply op, which adds the shortcut (in place over the downsample output) and
+// applies the ReLU.  The last block writes ASP's pooled frame [B][1][T'][F'*C] (feature f*C + c) directly; the ASP and
+// bottleneck weights are permuted on the host from the reference's feature order c*F' + f (x.reshape(B, C*F', T')).
+constexpr float kSimamLambda = 1e-4f;   // samresnet.py:65
+
+// out = relu(SimAM(y) + res), out at element b*os.b + f*os.f + t*os.t + c (y's extents); lvl: stride level of y
+static bool simam(Builder& b, const View& y, const View& res, const View& out, WsMapStrides os, float* partial, float* stats, int lvl) {
+    const View yv = y, rv = res;
+    void* op_ = out.p;
+    float* olo = (float*)out.plo;
+    const WsMapStrides rs{(long long)res.F * res.T * res.ld, (long long)res.T * res.ld, res.ld};
+    const int* l = b.lens(lvl);
+    const int dt = b.e.act_dt;
+    set_op_trace("{\"kind\":\"simam_stats\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", yv) + "," + Builder::tp("stats", stats) + "," +
+                 Builder::tp("lens", l) + "}");
+    b.push([=](cudaStream_t s) { return ws_launch_simam_stats(yv.p, dt, yv.B, yv.F, yv.T, yv.C, yv.ld, partial, stats, s, l); }, "simam_stats");
+    b.p.extra_launches += 1;   // partials + merge
+    set_op_trace("{\"kind\":\"simam_apply\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("y", yv) + "," + Builder::tp("stats", stats) + "," +
+                 Builder::tview("res", rv) + "," + Builder::tp("out", op_) + "," + Builder::ti("out_sb", os.b) + "," + Builder::ti("out_sf", os.f) + "," +
+                 Builder::ti("out_st", os.t) + "," + Builder::tp("lens", l) + ",\"lambda\":1e-4}");
+    b.push([=](cudaStream_t s) {
+        return ws_launch_simam_apply(yv.p, yv.ld, stats, kSimamLambda, rv.p, rs, op_, olo, os, dt, yv.B, yv.F, yv.T, yv.C, s, l);
+    }, "simam_apply");
+    return b.good();
+}
+
+// one SimAMBasicBlock (samresnet.py:57-63); x lives in none of hbuf / ybuf / obuf.  frame != nullptr: the trunk's last block,
+// whose output is the pooled frame (B,1,T',F'*C).  lvl: stride level of the block's output
+static View simam_block(Builder& b, const std::string& p, const View& x, int cout, int s, View hbuf, View ybuf, View obuf, int lvl,
+                        float* partial, float* stats, const View* frame) {
+    View none;
+    std::vector<float> s1, h1, s2, h2, w1, w2;
+    int co, ci, nt;
+    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co, &ci, &nt) ||
+        !b.w.pack_conv(p + ".conv2.weight", &s2, w2, &co, &ci, &nt))
+        return none;
+    const int Fo = (x.F - 1) / s + 1, To = (x.T - 1) / s + 1;
+    View h = hbuf; h.B = x.B; h.F = Fo; h.T = To; h.C = cout; h.ld = cout;
+    View y = ybuf; y.B = x.B; y.F = Fo; y.T = To; y.C = cout; y.ld = cout;
+    View o = obuf; o.B = x.B; o.F = Fo; o.T = To; o.C = cout; o.ld = cout;
+    if (!res2_conv3x3(b, p + ".conv1", x, nullptr, h, w1, h1, WS_ACT_RELU, s, lvl) || !res2_conv3x3(b, p + ".conv2", h, nullptr, y, w2, h2, WS_ACT_NONE, 1, lvl))
+        return none;
+    const bool has_ds = b.e.sd.count(p + ".downsample.0.weight") != 0;
+    if (has_ds) {
+        std::vector<float> ss, hs, wsv;
+        if (!b.w.bn(p + ".downsample.1", true, ss, hs) || !b.w.pack_conv(p + ".downsample.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
+        if (co != cout || ci != x.C || nt != 1) { set_err(p + ".downsample.0.weight: shape mismatch"); b.ok = false; return none; }
+        WsEpi es{};
+        es.bias = b.w.f32("bnh:" + p + ".downsample", hs);
+        b.conv_simple(x, o, b.w.act("w:" + p + ".downsample", wsv), 1, 1, 1, 1, 0, 0, s, s, es);
+        if (!b.good()) return none;
+    } else if (x.C != cout || s != 1) {
+        set_err(p + ": identity shortcut with a shape change"); b.ok = false; return none;
+    }
+    View dst = o;
+    WsMapStrides os{(long long)Fo * To * cout, (long long)To * cout, cout};
+    if (frame != nullptr) {
+        if (frame->T != To || frame->C != Fo * cout) { set_err("internal: pooled frame shape mismatch"); b.ok = false; return none; }
+        dst = *frame;
+        os = WsMapStrides{(long long)To * Fo * cout, cout, (long long)Fo * cout};
+    }
+    if (!simam(b, y, has_ds ? o : x, dst, os, partial, stats, lvl)) return none;
+    return dst;
+}
+
+bool build_simam_resnet(Builder& b) {
+    ws_engine& e = b.e;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim;
+    const HostT* c1 = b.w.get("front.conv1.weight");
+    if (c1 == nullptr) return false;
+    const int m = (int)c1->shape[0];   // in_planes
+    if (m != 32 && m != 64) { set_err("SimAM-ResNet: in_planes (the rows of front.conv1.weight) must be 32 or 64"); return false; }
+    // every map has F * C = feat_dim * in_planes (the stride-2 layers halve F and double C): a layer-1 tensor is the largest
+    const size_t big = (size_t)B * Fd * T * m;
+    View bufs[4];
+    for (int i = 0; i < 4; ++i) {
+        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
+        if (e.split) bufs[i].plo = b.raw(big * 4);
+    }
+    int F4 = Fd, T4 = T;
+    for (int i = 0; i < 3; ++i) { F4 = (F4 - 1) / 2 + 1; T4 = (T4 - 1) / 2 + 1; }
+    const int C4 = 8 * m, D = F4 * C4;   // ASP feature_dim = in_planes * 8 * (acoustic_dim / 8) (pooling_layers.py:167-170)
+    View frame = b.act(B, 1, T4, D);
+    float* partial = b.f32((size_t)B * Fd * m * 2);
+    float* sstats = b.f32((size_t)B * 2 * C4);
+    if (!b.good()) return false;
+    View cur = stem(b, "front.conv1.weight", "front.bn1", bufs[0]);
+    if (!b.good() || cur.p == nullptr) return false;
+    int ci = 0;
+    for (int li = 1; li <= 4; ++li)
+        for (int bi = 0; bi < e.num_blocks[li - 1]; ++bi) {
+            const bool last = li == 4 && bi == e.num_blocks[3] - 1;
+            View o = simam_block(b, "front.layer" + std::to_string(li) + "." + std::to_string(bi), cur, m << (li - 1), (bi == 0 && li > 1) ? 2 : 1,
+                                 bufs[(ci + 1) % 4], bufs[(ci + 2) % 4], bufs[(ci + 3) % 4], li - 1, partial, sstats, last ? &frame : nullptr);
+            if (!b.good() || o.p == nullptr) return false;
+            ci = (ci + 3) % 4;
+            cur = o;
+        }
+    // ASP (pooling_layers.py:180-204): attention.0 (Conv1d D -> 128, bias) -> ReLU -> attention.2 (BN) -> attention.3 (Conv1d
+    // 128 -> D) -> softmax over T; mean / sqrt(clamp(var, 1e-5)); then the bottleneck Linear(2D -> E)
+    const HostT* a0 = b.w.get("pooling.attention.0.weight");
+    const HostT* a3 = b.w.get("pooling.attention.3.weight");
+    const HostT* a3b = b.w.get("pooling.attention.3.bias");
+    const HostT* bw = b.w.get("bottleneck.weight");
+    std::vector<float> sa, ha;
+    if (!a0 || !a3 || !a3b || !bw || !b.w.bn("pooling.attention.2", true, sa, ha)) return false;
+    if (a0->numel() != 128LL * D || a3->numel() != 128LL * D || a3b->numel() != D || bw->shape.size() != 2 || (int)bw->shape[0] != E ||
+        bw->shape[1] != 2LL * D) {
+        set_err("SimAM-ResNet: pooling.attention / bottleneck shapes do not match in_planes * 8 * (feat_dim / 8) features");
+        return false;
+    }
+    auto ref_of = [&](int j) { return (j % C4) * F4 + j / C4; };   // pooled feature j = f*C4 + c -> reference feature c*F4 + f
+    std::vector<float> w0((size_t)128 * D), w3((size_t)D * 128), b3(D), wb((size_t)E * 2 * D);
+    for (int o = 0; o < 128; ++o)
+        for (int j = 0; j < D; ++j) w0[(size_t)o * D + j] = a0->v[(size_t)o * D + ref_of(j)];
+    for (int j = 0; j < D; ++j) {
+        memcpy(&w3[(size_t)j * 128], &a3->v[(size_t)ref_of(j) * 128], 128 * 4);
+        b3[j] = a3b->v[ref_of(j)];
+    }
+    for (int o = 0; o < E; ++o)
+        for (int j = 0; j < D; ++j) {
+            wb[(size_t)o * 2 * D + j] = bw->v[(size_t)o * 2 * D + ref_of(j)];
+            wb[(size_t)o * 2 * D + D + j] = bw->v[(size_t)o * 2 * D + D + ref_of(j)];
+        }
+    View hid = b.act(B, 1, T4, 128);
+    float* stats = b.f32((size_t)B * 2 * D);
+    if (!b.good()) return false;
+    WsEpi ep{};   // ECAPA's conv -> relu -> bn epilogue
+    ep.bias = b.w.vec("pooling.attention.0.bias");
+    ep.act1 = WS_ACT_RELU;
+    ep.scale = b.w.f32("bns:pooling.attention.2", sa);
+    ep.shift = b.w.f32("bnh:pooling.attention.2", ha);
+    b.conv_simple(frame, hid, b.w.act("w:pooling.attention.0", w0), 1, 1, 1, 1, 0, 0, 1, 1, ep);
+    const void* W3 = b.w.act("w:pooling.attention.3", w3);
+    const int* l3 = b.lens(3);
+    bool fused = false;
+    if (e.use_tc >= 2 && e.opt("astp_fused", 1) && b.good()) {   // attention.3's bias cancels in the softmax
+        Op op;
+        bool unsupported = false;
+        if (make_astp_op(frame, hid, W3, stats, 1e-5f, &op, &unsupported, l3)) { b.push(std::move(op)); fused = true; }
+        else if (!unsupported) return false;
+    }
+    if (!fused) {
+        View logits = b.act(B, 1, T4, D);
+        WsEpi ep3{};
+        ep3.bias = b.w.f32("b:pooling.attention.3", b3);
+        b.conv_simple(hid, logits, W3, 1, 1, 1, 1, 0, 0, 1, 1, ep3);
+        if (!b.good()) return false;
+        const View fr = frame, lg = logits;
+        set_op_trace("{\"kind\":\"astp_stats\"," + Builder::ti("es", ws_esize(fr.dt)) + "," + Builder::tview("x", fr) + "," + Builder::tview("logits", lg) + "," +
+                     Builder::tp("stats", stats) + "," + Builder::tp("lens", l3) + ",\"eps\":1e-05}");
+        b.push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, B, T4, D, fr.ld, stats, 1e-5f, s, l3); }, "astp_stats");
+    }
+    b.linear(stats, 2 * D, nullptr, 0, 1, b.w.f32("w:bottleneck.pooled", wb), b.w.vec("bottleneck.bias"), b.p.emb, E, B, 2 * D, E, WS_ACT_NONE);
+    return b.good();
 }
 
 // ----------------------------------------------------------------------------------------------- XVEC
@@ -1535,6 +1696,7 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
         if (e->model.rfind("ECAPA", 0) == 0) ok = build_ecapa(b);
         else if (e->model.rfind("ResNet", 0) == 0) ok = build_resnet(b);
         else if (e->model == "XVEC") ok = build_xvec(b);
+        else if (e->model.rfind("SimAM_ResNet", 0) == 0) ok = build_simam_resnet(b);
         else if (e->r2_m != 0) {
             Res2Cfg c;
             c.m = e->r2_m; c.base_width = e->r2_base_width; c.scale = e->r2_scale; c.expansion = e->r2_expansion; c.fuse = e->r2_fuse;
@@ -1706,6 +1868,8 @@ static int configure_engine(ws_engine* e, const char* model_name, const char* pr
     else if (m == "ERes2Net34_Large") { e->num_blocks = {3, 4, 6, 3}; e->r2_m = 64; e->r2_fuse = true; }
     else if (m == "ERes2Net34_aug") { e->num_blocks = {3, 4, 6, 3}; e->r2_m = 64; e->r2_fuse = true; e->r2_base_width = 24; e->r2_scale = 3; e->r2_expansion = 4; }
     else if (m == "CAMPPlus") {}
+    else if (m == "SimAM_ResNet34_ASP") e->num_blocks = {3, 4, 6, 3};
+    else if (m == "SimAM_ResNet100_ASP") e->num_blocks = {6, 16, 24, 3};
     else { set_err("unknown / out-of-scope model name: " + m); return 1; }
     const std::string p = e->prec;
     if (p == "fp32") { e->act_dt = WS_F32; e->use_tc = 0; }

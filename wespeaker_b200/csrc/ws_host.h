@@ -101,10 +101,11 @@ void fill_epi_out(WsEpi& e, const View& out);
 bool make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
                   const float* shift, int w8, int dil, Op* op, bool* unsupported, const int* lens = nullptr);
 
-// Fused ASTP tail (ws_astp_fused.cu): x = frame-level features (B,1,T,C), h = tanh(linear1(x)) (B,1,T,128), W2 = linear2 weight
-// [C][128] in the activation dtype, stats = fp32 [B][2C] (weighted mean, std).  linear2's bias cancels in the softmax over
-// time and is not needed.  *unsupported = true outside the envelope (fp32 activations, C % 128, hidden width != 128).
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, Op* op, bool* unsupported,
+// Fused ASTP tail (ws_astp_fused.cu): x = frame-level features (B,1,T,C), h = the attention's hidden layer (B,1,T,128), W2 =
+// linear2 weight [C][128] in the activation dtype, stats = fp32 [B][2C] (weighted mean, std = sqrt(max(var, var_floor))).
+// linear2's bias cancels in the softmax over time and is not needed.  *unsupported = true outside the envelope (fp32
+// activations, C % 128, hidden width != 128).
+bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, Op* op, bool* unsupported,
                   const int* lens = nullptr);
 
 // Halo-resident 3x3 pad-1 conv (ws_conv3x3.cu), strides 1 or 2 per axis: out = act(conv(x, W) + bias [+ res]).  x/out/res:

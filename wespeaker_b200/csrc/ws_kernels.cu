@@ -381,7 +381,7 @@ __global__ void aff_combine_kernel(const void* __restrict__ x, long long x_ld, c
 // sums rescaled by exp(m_old - m_new); the 8 T-slices are merged through shared memory.
 __global__ void __launch_bounds__(256) astp_stats_kernel(const void* __restrict__ x, const void* __restrict__ lg,
                                                          int dt, int T, int C, long long ld, float* __restrict__ out,
-                                                         const int* __restrict__ lens) {
+                                                         float var_floor, const int* __restrict__ lens) {
     __shared__ float red[4][8][65];
     const int c = (blockIdx.x * 32 + threadIdx.x) * 2;
     const int b = blockIdx.y;
@@ -431,7 +431,7 @@ __global__ void __launch_bounds__(256) astp_stats_kernel(const void* __restrict_
             const float mean = a1 / a0;
             const float var = a2 / a0 - mean * mean;
             out[(long long)b * 2 * C + cc] = mean;
-            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, 1e-7f));
+            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, var_floor));
         }
     }
 }
@@ -444,7 +444,7 @@ __global__ void __launch_bounds__(256) astp_stats_kernel(const void* __restrict_
 template <int dt>
 __global__ void __launch_bounds__(512, 2) astp_stats4_kernel(const void* __restrict__ x, const void* __restrict__ lg,
                                                              int T, int C, long long ld, float* __restrict__ out,
-                                                             const int* __restrict__ lens) {
+                                                             float var_floor, const int* __restrict__ lens) {
     __shared__ float red[16][4][64];
     const int cg = threadIdx.x, sl = threadIdx.y, warp = sl >> 1;   // a warp = 2 slices x 16 channel groups
     const int c = (blockIdx.x * 16 + cg) * 4;
@@ -527,7 +527,7 @@ __global__ void __launch_bounds__(512, 2) astp_stats4_kernel(const void* __restr
             const float mean = a1 / a0;
             const float var = a2 / a0 - mean * mean;
             out[(long long)b * 2 * C + cc] = mean;
-            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, 1e-7f));
+            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, var_floor));
         }
     }
 }
@@ -967,17 +967,17 @@ const char* ws_launch_aff_combine(const void* x, long long x_ld, const void* y, 
 }
 
 const char* ws_launch_astp_stats(const void* x, const void* logits, int dt, int B, int T, int C, long long ld,
-                                 float* out, cudaStream_t s, const int* lens) {
+                                 float* out, float var_floor, cudaStream_t s, const int* lens) {
     if (C % 2 != 0) return "astp_stats: C must be even";
     static const int variant = getenv("WS_ASTP_VARIANT") ? atoi(getenv("WS_ASTP_VARIANT")) : 2;
     if (variant == 2 && C % 4 == 0 && ld % 4 == 0 && dt != WS_F32 && T <= 256) {
         dim3 grid((C + 63) / 64, B), block(16, 32);
-        if (dt == WS_BF16) astp_stats4_kernel<WS_BF16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, lens);
-        else astp_stats4_kernel<WS_F16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, lens);
+        if (dt == WS_BF16) astp_stats4_kernel<WS_BF16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);
+        else astp_stats4_kernel<WS_F16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);
         return last_err();
     }
     dim3 grid((C + 63) / 64, B), block(32, 8);
-    astp_stats_kernel<<<grid, block, 0, s>>>(x, logits, dt, T, C, ld, out, lens);
+    astp_stats_kernel<<<grid, block, 0, s>>>(x, logits, dt, T, C, ld, out, var_floor, lens);
     return last_err();
 }
 

@@ -30,9 +30,23 @@ const char* ws_launch_scale_residual(const void* x, long long x_ld, const float*
 // ERes2Net AFF combine (eres2net.py:97-100): out[pos][c] = x * (1 + t) + y * (2 - (1 + t)), t = the tanh'd attention map
 const char* ws_launch_aff_combine(const void* x, long long x_ld, const void* y, long long y_ld, const void* t, long long t_ld,
                                   void* out, float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s);
-// ASTP statistics (pooling_layers.py:138-144): softmax over T of logits, weighted mean / std of x
+// ASTP statistics (pooling_layers.py:138-144): softmax over T of logits, weighted mean / std = sqrt(max(var, var_floor)) of x
+// (ECAPA's ASTP floors the variance at 1e-7, SimAM-ResNet's ASP at 1e-5, pooling_layers.py:198-203)
 const char* ws_launch_astp_stats(const void* x, const void* logits, int dt, int B, int T, int C, long long ld,
-                                 float* out /*[B][2C]*/, cudaStream_t s, const int* lens = nullptr);
+                                 float* out /*[B][2C]*/, float var_floor, cudaStream_t s, const int* lens = nullptr);
+// SimAM (ws_simam.cu, samresnet.py:65-70).  Statistics of y [B][F][T][ld] (channels [0,C)) per (b, c) over F x (its own
+// frames): stats fp32 [B][2][C] = mean, variance over n = F*T_b - 1; partial: fp32 scratch [B][F][C][2] (two launches).
+const char* ws_launch_simam_stats(const void* y, int dt, int B, int F, int T, int C, long long ld, float* partial, float* stats,
+                                  cudaStream_t s, const int* lens = nullptr);
+// element (b, f, t, c) of a map at b*sb.b + f*sb.f + t*sb.t + c (elements)
+struct WsMapStrides {
+    long long b, f, t;
+};
+// out = relu(y * sigmoid((y - mean)^2 / (4 (var + lambda_p)) + 0.5) + res); res may alias out; rows t >= lens[b] of out are
+// zeroed; out_lo (optional, fp32 with out's strides) receives the 3xTF32 low part
+const char* ws_launch_simam_apply(const void* y, long long y_ld, const float* stats, float lambda_p, const void* res, WsMapStrides rs,
+                                  void* out, float* out_lo, WsMapStrides os, int dt, int B, int F, int T, int C, cudaStream_t s,
+                                  const int* lens = nullptr);
 // out[pos][c] = relu(x[pos][c]*scale[c] + shift[c])  (CAM++ pre-activation BN-ReLU, campplus.py:164-166,214)
 const char* ws_launch_bnrelu(const void* x, long long x_ld, const float* scale, const float* shift, void* out,
                              float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s);

@@ -34,6 +34,17 @@ class ConvDesc(C.Structure):
     ]
 
 
+class SimamDesc(C.Structure):
+    """ws_simam_desc (include/wespeaker_b200.h)."""
+    _fields_ = [
+        ("y", C.c_void_p), ("y_ld", C.c_longlong), ("B", C.c_int), ("F", C.c_int), ("T", C.c_int), ("C", C.c_int),
+        ("lens", C.c_void_p), ("lambda_p", C.c_float), ("res", C.c_void_p), ("res_sb", C.c_longlong),
+        ("res_sf", C.c_longlong), ("res_st", C.c_longlong), ("out", C.c_void_p), ("out_sb", C.c_longlong),
+        ("out_sf", C.c_longlong), ("out_st", C.c_longlong), ("out_lo", C.c_void_p), ("dtype", C.c_int),
+        ("stats", C.c_void_p), ("partial", C.c_void_p),
+    ]
+
+
 _PROTOS = {
     "ws_version": (C.c_int, []),
     "ws_last_error": (C.c_char_p, []),
@@ -74,6 +85,7 @@ _PROTOS = {
     "ws_fbank": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_void_p,
                            C.c_void_p]),
     "ws_conv": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
+    "ws_simam": (C.c_int, [C.POINTER(SimamDesc), C.c_void_p]),
     "ws_plda_create": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                  C.POINTER(c_plda_p)]),
     "ws_plda_transform": (C.c_int, [c_plda_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -20,11 +20,12 @@ import numpy as np
 import torch
 
 from . import lib as _lib
-from .synthetic import (CAMPP_NAMES, DEFAULT_MODEL_ARGS, ECAPA_NAMES, RES2NET_NAMES, RESNET_NAMES, XVEC_NAMES,
+from .synthetic import (CAMPP_NAMES, DEFAULT_MODEL_ARGS, ECAPA_NAMES, RES2NET_NAMES, RESNET_NAMES, SIMAM_NAMES, XVEC_NAMES,
                         state_dict_spec)
 
 _IncompatibleKeys = namedtuple("IncompatibleKeys", ["missing_keys", "unexpected_keys"])
-SUPPORTED_MODELS = tuple(ECAPA_NAMES) + tuple(RESNET_NAMES) + tuple(CAMPP_NAMES) + tuple(XVEC_NAMES) + tuple(RES2NET_NAMES)
+SUPPORTED_MODELS = tuple(ECAPA_NAMES) + tuple(RESNET_NAMES) + tuple(CAMPP_NAMES) + tuple(XVEC_NAMES) + tuple(RES2NET_NAMES) \
+    + tuple(SIMAM_NAMES)
 
 
 class B200SpeakerModel(torch.nn.Module):
@@ -44,7 +45,8 @@ class B200SpeakerModel(torch.nn.Module):
         self.model_name = model_name
         self.model_args = args
         self.precision = precision or os.environ.get("WESPEAKER_B200_PRECISION", "tf32x3")
-        self.feat_dim = int(args["feat_dim"])
+        # SimAM-ResNet names its feature dimension acoustic_dim (samresnet.py:135)
+        self.feat_dim = int(args["acoustic_dim"] if model_name in SIMAM_NAMES else args["feat_dim"])
         self.embed_dim = int(args["embed_dim"])
         self._spec = state_dict_spec(model_name, **args)
         self._sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
@@ -221,8 +223,8 @@ class B200SpeakerModel(torch.nn.Module):
 
     def forward(self, features: torch.Tensor):
         emb = self.embed(features)
-        if self.model_name in CAMPP_NAMES or self.model_name in RES2NET_NAMES:
-            return emb  # campplus.py:409-413, res2net.py:199, eres2net.py:391 return a bare tensor
+        if self.model_name in CAMPP_NAMES or self.model_name in RES2NET_NAMES or self.model_name in SIMAM_NAMES:
+            return emb  # campplus.py:409-413, res2net.py:199, eres2net.py:391, samresnet.py:142-149 return a bare tensor
         # ecapa_tdnn.py:234 returns (out4, emb); resnet.py:204 returns (tensor(0.), embed_a).  Callers use [-1].
         return torch.tensor(0.0), emb
 

@@ -47,6 +47,8 @@ RES2NET_NAMES = {
     "ERes2Net34_Large": dict(m_channels=64, num_blocks=[3, 4, 6, 3], base_width=32, scale=2, expansion=2, fuse=True),
     "ERes2Net34_aug": dict(m_channels=64, num_blocks=[3, 4, 6, 3], base_width=24, scale=3, expansion=4, fuse=True),
 }
+# SimAM-ResNet with ASP pooling, the VoxBlink2 models (`wespeaker/models/samresnet.py:126-167`): block counts
+SIMAM_NAMES = {"SimAM_ResNet34_ASP": [3, 4, 6, 3], "SimAM_ResNet100_ASP": [6, 16, 24, 3]}
 
 DEFAULT_MODEL_ARGS = {
     # examples/voxceleb/v2/conf/{ecapa_tdnn,resnet,campplus}.yaml
@@ -69,6 +71,9 @@ DEFAULT_MODEL_ARGS = {
     "ERes2Net34_Base": dict(feat_dim=80, embed_dim=512, pooling_func="TSTP", two_emb_layer=False),
     "ERes2Net34_Large": dict(feat_dim=80, embed_dim=512, pooling_func="TSTP", two_emb_layer=False),
     "ERes2Net34_aug": dict(feat_dim=80, embed_dim=512, pooling_func="TSTP", two_emb_layer=False),
+    # the reference constructor's own arguments (samresnet.py:135): no feat_dim, the feature dimension is acoustic_dim
+    "SimAM_ResNet34_ASP": dict(in_planes=64, embed_dim=256, acoustic_dim=80, dropout=0),
+    "SimAM_ResNet100_ASP": dict(in_planes=64, embed_dim=256, acoustic_dim=80, dropout=0),
 }
 
 
@@ -300,6 +305,38 @@ def res2net_spec(m_channels=32, num_blocks=(3, 4, 6, 3), base_width=32, scale=2,
     return s
 
 
+def simam_spec(num_blocks, in_planes=64, embed_dim=256, acoustic_dim=80, dropout=0):
+    """`wespeaker/models/samresnet.py:21-167`: the ResNet trunk under ``front.`` (SimAMBasicBlock: conv1/bn1, conv2/bn2, and a
+    ``downsample`` Sequential of a strided 1x1 conv and a BN where the shape changes), ASP pooling (`pooling_layers.py:151-186`:
+    Conv1d -> ReLU -> BN -> Conv1d over in_planes * 8 * int(acoustic_dim / 8) features) and the ``bottleneck`` Linear.
+    ``dropout`` only acts in training."""
+    s = OrderedDict()
+    s["front.conv1.weight"] = (in_planes, 1, 3, 3)
+    _bn(s, "front.bn1", in_planes)
+    cin = in_planes
+    for li, (nb, mult, stride) in enumerate(zip(num_blocks, (1, 2, 4, 8), (1, 2, 2, 2)), 1):
+        planes = in_planes * mult
+        for bi in range(nb):
+            p = f"front.layer{li}.{bi}"
+            s[f"{p}.conv1.weight"] = (planes, cin, 3, 3)
+            _bn(s, f"{p}.bn1", planes)
+            s[f"{p}.conv2.weight"] = (planes, planes, 3, 3)
+            _bn(s, f"{p}.bn2", planes)
+            if (stride if bi == 0 else 1) != 1 or cin != planes:
+                s[f"{p}.downsample.0.weight"] = (planes, cin, 1, 1)
+                _bn(s, f"{p}.downsample.1", planes)
+            cin = planes
+    feature_dim = in_planes * 8 * int(acoustic_dim / 8)
+    s["pooling.attention.0.weight"] = (128, feature_dim, 1)
+    s["pooling.attention.0.bias"] = (128,)
+    _bn(s, "pooling.attention.2", 128)
+    s["pooling.attention.3.weight"] = (feature_dim, 128, 1)
+    s["pooling.attention.3.bias"] = (feature_dim,)
+    s["bottleneck.weight"] = (embed_dim, 2 * feature_dim)
+    s["bottleneck.bias"] = (embed_dim,)
+    return s
+
+
 def state_dict_spec(model_name: str, **model_args):
     """key -> shape for a reference model name (`wespeaker/models/speaker_model.py:31-62`)."""
     if model_name in ECAPA_NAMES:
@@ -312,6 +349,8 @@ def state_dict_spec(model_name: str, **model_args):
         return res2net_spec(**RES2NET_NAMES[model_name], **model_args)
     if model_name in CAMPP_NAMES:
         return campplus_spec(**model_args)
+    if model_name in SIMAM_NAMES:
+        return simam_spec(SIMAM_NAMES[model_name], **model_args)
     raise ValueError(f"model {model_name!r} is not on the engine's hot path")
 
 
@@ -334,7 +373,8 @@ def make_state_dict(model_name: str, seed: int = 0, **model_args):
         elif key.endswith("running_var"):
             sd[key] = g.uniform(0.5, 1.5, shape).astype(np.float32)
         elif ".bn" in key or "batchnorm" in key or key.startswith("bn") or "shortcut.1" in key \
-                or "seg_bn" in key or "local_att.1." in key or "local_att.4." in key:
+                or "seg_bn" in key or "local_att.1." in key or "local_att.4." in key or "downsample.1." in key \
+                or "pooling.attention.2." in key:
             if (key.endswith(".bn2.weight") or key.endswith(".bn3.weight")) and "layer" in key:
                 # residual-branch output BN of the 2-D BasicBlocks: keep the residual sum O(1)
                 # over 16 blocks (a trained net does; fp16 range matters for config 3)
