@@ -27,7 +27,8 @@ const char* ws_last_error(void);
  * model_name: ECAPA_TDNN_c512 | ECAPA_TDNN_GLOB_c512 | ECAPA_TDNN_c1024 | ECAPA_TDNN_GLOB_c1024 | ResNet18 |
  *             ResNet34 | CAMPPlus; SURVEY section 8(f) rank 4: ResNet50 | ResNet101 | ResNet152 | ResNet221 | ResNet293 |
  *             XVEC | Res2Net34_Base | Res2Net34_Large | ERes2Net34_Base | ERes2Net34_Large | ERes2Net34_aug |
- *             SimAM_ResNet34_ASP | SimAM_ResNet100_ASP.
+ *             SimAM_ResNet34_ASP | SimAM_ResNet100_ASP | Gemini_DF_ResNet60 | Gemini_DF_ResNet114 | Gemini_DF_ResNet183 |
+ *             Gemini_DF_ResNet237.
  * precision:  "fp32" (exact IEEE fp32 FFMA path, parity <= 1e-4), "tf32x3" (tensor cores with 3xTF32 error compensation,
  *             fp32-grade accuracy), "tf32", "bf16", "fp16" (wgmma tensor cores). */
 int ws_engine_create(const char* model_name, const char* precision, int feat_dim, int embed_dim, int device,
@@ -172,6 +173,24 @@ typedef struct {
     float* partial;           /* fp32 scratch [B][F][C][2] */
 } ws_simam_desc;
 int ws_simam(const ws_simam_desc* d, void* stream);
+
+/* ---- depthwise 3x3 conv + folded BN + ReLU of a Gemini DF-ResNet block (gemini_dfresnet.py:30-48), exported for parity
+ *      tests: out[b,f,t,c] = relu(sum_{df,dt} w[c][df+1][dt+1] * x[b,f+df,t+dt,c] + shift[c]), zero padding outside
+ *      [0,F) x [0,T_b).  fp32 accumulation in a fixed tap order, one rounding to the activation dtype.  Element (b, f, t, c)
+ *      of x / out is at ((b*F + f)*T + t)*ld + c.  All pointers are device pointers, 16-byte aligned. */
+typedef struct {
+    const void* x;            /* [B][F][T][x_ld], channels [0,C), dtype below; C % 8 == 0 (16-bit) or C % 4 == 0 (fp32) */
+    long long x_ld;
+    int B, F, T, C;
+    const int* lens;          /* int32[B] frames per utterance (rows t >= lens[b] are read as zeros and written as zeros) or NULL */
+    const float* w;           /* fp32 [C][3][3], the BN scale folded in */
+    const float* shift;       /* fp32 [C] */
+    void* out;                /* [B][F][T][out_ld] */
+    long long out_ld;
+    void* out_lo;             /* dtype 0 only, optional: fp32 out - tf32_trunc(out) with out's layout */
+    int dtype;                /* 0 fp32, 1 bf16, 2 fp16 */
+} ws_dwconv_desc;
+int ws_dwconv(const ws_dwconv_desc* d, void* stream);
 
 /* ---- two-covariance PLDA scorer: replaces TwoCovPLDA.transform_embedding / log_likelihood_ratio / the trial
  *      loop of eval_sv (wespeaker/utils/plda/two_cov_plda.py:156-184,186-256), fp64 like the reference. */

@@ -810,12 +810,13 @@ View stem(Builder& b, const std::string& convkey, const std::string& bnkey, View
 
 // TSTP over the last feature map + the segment layer(s) (resnet.py:187-204; the same tail closes Res2Net / ERes2Net,
 // res2net.py:186-199, eres2net.py:379-391)
-bool resnet_tail(Builder& b, const View& cur, int E) {
+// lvl: stride level of `cur` in length-masked plans (three stride-2 layers in ResNet / Res2Net, one in Gemini DF-ResNet)
+bool resnet_tail(Builder& b, const View& cur, int E, int lvl = 3) {
     ws_engine& e = b.e;
     const int B = b.p.B;
     const int sd = cur.C * cur.F;  // stats_dim
     float* stats = b.f32((size_t)B * 2 * sd);
-    b.tstats(cur, nullptr, nullptr, stats, 2 * sd, sd, 3);  // TSTP, index c*F' + f (pooling_layers.py:78-85); stride level 3
+    b.tstats(cur, nullptr, nullptr, stats, 2 * sd, sd, lvl);  // TSTP, index c*F' + f (pooling_layers.py:78-85)
     const HostT* w1 = b.w.get("seg_1.weight");
     if (!w1) return false;
     if ((int)w1->shape[1] != 2 * sd || (int)w1->shape[0] != E) { set_err("seg_1.weight shape mismatch"); return false; }
@@ -972,17 +973,18 @@ static bool aff(Builder& b, const std::string& p, const View& x, const View& y, 
 
 // 3x3 pad-1 conv (+ folded BN shift) -> act over `in` (and, when in2 != nullptr, over in + in2 with the weights repeated):
 // the halo-resident kernel where it applies, else the generic conv-GEMM.  act: WS_ACT_RELU20, WS_ACT_RELU or WS_ACT_NONE.
+// stride_t: the time stride when it differs from the frequency stride `stride` (0: the same)
 static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, const View* in2, const View& out, const std::vector<float>& w9,
-                         const std::vector<float>& bias, int act, int stride, int lvl) {   // lvl: stride level of `out` (length-masked plans)
-    const int Cin = in.C, Cout = out.C;
+                         const std::vector<float>& bias, int act, int stride, int lvl, int stride_t = 0) {   // lvl: stride level of `out` (length-masked plans)
+    const int Cin = in.C, Cout = out.C, sf = stride, st = stride_t > 0 ? stride_t : stride;
     if ((int)w9.size() != Cout * 9 * Cin || (int)bias.size() != Cout) { set_err(id + ": 3x3 weight shape mismatch"); b.ok = false; return false; }
     const float* bd = b.w.f32("b:" + id, bias);
     if (in2 == nullptr) {
         const void* W = b.w.act("w:" + id, w9);
-        if (b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0 && (stride == 1 || b.e.opt("conv3x3_strided", 1) != 0)) {
+        if (b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0 && ((sf == 1 && st == 1) || b.e.opt("conv3x3_strided", 1) != 0)) {
             Op op;
             bool unsupported = false;
-            if (make_conv3x3_op(in, out, W, bd, nullptr, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, &op, &unsupported, stride, stride,
+            if (make_conv3x3_op(in, out, W, bd, nullptr, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, &op, &unsupported, sf, st,
                                 b.lens(lvl))) {
                 b.push(std::move(op));
                 return b.good();
@@ -992,7 +994,7 @@ static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, cons
         WsEpi ep{};
         ep.bias = bd;
         ep.act1 = act;
-        b.conv_simple(in, out, W, 3, 3, 1, 1, 1, 1, stride, stride, ep);
+        b.conv_simple(in, out, W, 3, 3, 1, 1, 1, 1, sf, st, ep);
         b.zero_tail(out, lvl);
         return b.good();
     }
@@ -1005,8 +1007,8 @@ static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, cons
     ConvSpec cs;
     cs.dt = b.e.act_dt;
     int Fo, To, F2, T2;
-    const int K1 = add_conv_taps(cs, in, 3, 3, 1, 1, 1, 1, stride, stride, 0, &Fo, &To);
-    const int K2 = K1 < 0 ? -1 : add_conv_taps(cs, *in2, 3, 3, 1, 1, 1, 1, stride, stride, K1, &F2, &T2);
+    const int K1 = add_conv_taps(cs, in, 3, 3, 1, 1, 1, 1, sf, st, 0, &Fo, &To);
+    const int K2 = K1 < 0 ? -1 : add_conv_taps(cs, *in2, 3, 3, 1, 1, 1, 1, sf, st, K1, &F2, &T2);
     if (K1 != 9 * Cin || K2 != 9 * Cin || Fo != out.F || To != out.T || F2 != Fo || T2 != To) { set_err(id + ": summed-input conv shape mismatch"); b.ok = false; return false; }
     cs.W = b.w.act("w:" + id + ".x2", w2); cs.Ktot = 18 * Cin; cs.Cout = Cout; cs.B = out.B; cs.F = Fo; cs.T = To;
     cs.epi.bias = bd;
@@ -1340,6 +1342,130 @@ bool build_simam_resnet(Builder& b) {
     }
     b.linear(stats, 2 * D, nullptr, 0, 1, b.w.f32("w:bottleneck.pooled", wb), b.w.vec("bottleneck.bias"), b.p.emb, E, B, 2 * D, E, WS_ACT_NONE);
     return b.good();
+}
+
+// ----------------------------------------------------------------------------------------------- Gemini DF-ResNet
+// gemini_dfresnet.py:30-176: the stem (downsample_layers.0: 3x3 conv + BN + ReLU), four 3x3 downsample convs + BN (no ReLU)
+// with frequency stride 2 and time strides (1, 2, 1, 1), each followed by a stage of inverted bottlenecks (1x1 expand to
+// 4 dim + BN + ReLU, depthwise 3x3 + BN + ReLU, 1x1 project + BN, + x, ReLU), TSTP and the segment layer(s) of ResNet.
+// Every BN is folded into its conv.  The expand and project convs are 1x1 conv-GEMMs (the residual and the final ReLU in
+// the project conv's epilogue), the depthwise conv is its own bandwidth kernel (ws_dwconv.cu) and the downsample convs
+// run on res2_conv3x3 (the halo-resident kernel where the channels allow, else the conv-GEMM).
+constexpr int kGeminiStrideT[4] = {1, 2, 1, 1};   // gemini_dfresnet.py:74-75 (the frequency stride is 2 in all four)
+
+// out = relu(depthwise 3x3(x, w9) + shift); rows behind an utterance's end read and written as zeros.  lvl: stride level of x
+static bool dwconv3x3(Builder& b, const std::string& id, const View& x, const View& out, const float* w9, const float* shift, int lvl) {
+    const int V = x.dt == WS_F32 ? 4 : 8;
+    if (x.C % V != 0 || x.ld % V != 0 || out.ld % V != 0 || out.C != x.C || out.B != x.B || out.F != x.F || out.T != x.T) {
+        set_err(id + ": the depthwise conv needs a channel count that is a multiple of " + std::to_string(V) + " (got " + std::to_string(x.C) + ")");
+        b.ok = false;
+        return false;
+    }
+    const View xv = x, ov = out;
+    const int* l = b.lens(lvl);
+    set_op_trace("{\"kind\":\"dwconv3x3\"," + Builder::ti("es", ws_esize(xv.dt)) + "," + Builder::tview("x", xv) + "," + Builder::tview("out", ov) + "," +
+                 Builder::tp("w", w9) + "," + Builder::tp("shift", shift) + "," + Builder::tp("lens", l) + "}");
+    b.push([=](cudaStream_t s) {
+        return ws_launch_dwconv3x3(xv.p, xv.ld, w9, shift, ov.p, (float*)ov.plo, ov.ld, xv.dt, xv.B, xv.F, xv.T, xv.C, s, l);
+    }, "dwconv3x3");
+    return b.good();
+}
+
+// one Inverted_Bottleneck (gemini_dfresnet.py:30-48); x lives in none of hbuf / dbuf / obuf.  lvl: stride level of x
+static View gemini_block(Builder& b, const std::string& p, const View& x, View hbuf, View dbuf, View obuf, int lvl) {
+    View none;
+    std::vector<float> s1, h1, s2, h2, s3, h3, w1, w3;
+    int co1, ci1, nt1, co3, ci3, nt3;
+    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.bn(p + ".bn3", true, s3, h3) ||
+        !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co1, &ci1, &nt1) || !b.w.pack_conv(p + ".conv3.weight", &s3, w3, &co3, &ci3, &nt3))
+        return none;
+    const HostT* c2 = b.w.get(p + ".conv2.weight");
+    if (c2 == nullptr) return none;
+    const int C4 = 4 * x.C;
+    if (co1 != C4 || ci1 != x.C || nt1 != 1 || co3 != x.C || ci3 != C4 || nt3 != 1 || c2->shape.size() != 4 || c2->shape[0] != C4 ||
+        c2->shape[1] != 1 || c2->numel() != 9LL * C4 || (int)s2.size() != C4) {
+        set_err(p + ": inverted bottleneck weights do not match dim " + std::to_string(x.C));
+        b.ok = false;
+        return none;
+    }
+    std::vector<float> w2((size_t)C4 * 9);   // [C4][3][3] with bn2's scale folded in
+    for (int c = 0; c < C4; ++c)
+        for (int k = 0; k < 9; ++k) w2[(size_t)c * 9 + k] = c2->v[(size_t)c * 9 + k] * s2[c];
+    View h = hbuf; h.B = x.B; h.F = x.F; h.T = x.T; h.C = C4; h.ld = C4;
+    View d = dbuf; d.B = x.B; d.F = x.F; d.T = x.T; d.C = C4; d.ld = C4;
+    View o = obuf; o.B = x.B; o.F = x.F; o.T = x.T; o.C = x.C; o.ld = x.C;
+    WsEpi e1{};
+    e1.bias = b.w.f32("bnh:" + p + ".bn1", h1);
+    e1.act1 = WS_ACT_RELU;
+    b.conv_simple(x, h, b.w.act("w:" + p + ".conv1", w1), 1, 1, 1, 1, 0, 0, 1, 1, e1);
+    if (!b.good() || !dwconv3x3(b, p + ".conv2", h, d, b.w.f32("w:" + p + ".conv2", w2), b.w.f32("bnh:" + p + ".bn2", h2), lvl)) return none;
+    WsEpi e3{};
+    e3.bias = b.w.f32("bnh:" + p + ".bn3", h3);
+    e3.res = x.p;
+    e3.res_ld = x.ld;
+    e3.act2 = WS_ACT_RELU;
+    b.conv_simple(d, o, b.w.act("w:" + p + ".conv3", w3), 1, 1, 1, 1, 0, 0, 1, 1, e3);
+    if (!b.good()) return none;
+    return o;
+}
+
+bool build_gemini(Builder& b) {
+    ws_engine& e = b.e;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim;
+    int dims[5], Fs[5], Ts[5];
+    Fs[0] = Fd; Ts[0] = T;
+    for (int i = 0; i < 5; ++i) {
+        const std::string key = "downsample_layers." + std::to_string(i) + ".0.weight";
+        const HostT* w = b.w.get(key);
+        if (w == nullptr) return false;
+        if (w->shape.size() != 4 || w->shape[2] != 3 || w->shape[3] != 3 || w->shape[1] != (i == 0 ? 1 : dims[i - 1])) {
+            set_err(key + ": expected a (dim, previous dim, 3, 3) conv");
+            return false;
+        }
+        dims[i] = (int)w->shape[0];
+        if (i > 0) { Fs[i] = (Fs[i - 1] - 1) / 2 + 1; Ts[i] = (Ts[i - 1] - 1) / kGeminiStrideT[i - 1] + 1; }
+    }
+    // the reference sizes TSTP and seg_1 for stats_dim = int(feat_dim / 8 / 2) * dims[4] (gemini_dfresnet.py:62)
+    if (Fs[4] != Fd / 16) {
+        set_err("Gemini_DF_ResNet: feat_dim " + std::to_string(Fd) + " leaves " + std::to_string(Fs[4]) +
+                " frequency rows after the four stride-2 convs, but the reference's stats_dim = int(feat_dim / 16) * " + std::to_string(dims[4]) +
+                " expects " + std::to_string(Fd / 16));
+        return false;
+    }
+    // the largest map: the stem output or a stage's 4x-expanded tensor
+    size_t big = (size_t)Fd * T * dims[0];
+    for (int i = 1; i <= 4; ++i) big = std::max(big, (size_t)Fs[i] * Ts[i] * 4 * dims[i]);
+    big *= B;
+    View bufs[4];
+    for (int i = 0; i < 4; ++i) {
+        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
+        if (e.split) bufs[i].plo = b.raw(big * 4);
+    }
+    if (!b.good()) return false;
+    View cur = stem(b, "downsample_layers.0.0.weight", "downsample_layers.0.1", bufs[0]);
+    if (!b.good() || cur.p == nullptr) return false;
+    int ci = 0;
+    for (int i = 1; i <= 4; ++i) {
+        const std::string p = "downsample_layers." + std::to_string(i);
+        std::vector<float> s, h, w;
+        int co, cin, nt;
+        if (!b.w.bn(p + ".1", true, s, h) || !b.w.pack_conv(p + ".0.weight", &s, w, &co, &cin, &nt)) return false;
+        // stride levels of length-masked plans: 0 up to downsample_layers.2 (the only time stride), 1 behind it
+        const int lvl_in = i >= 3 ? 1 : 0, lvl = i >= 2 ? 1 : 0;
+        if (i >= 2) b.zero_tail(cur, lvl_in);   // (masked plans) a stage output, read across time by the 3x3 conv
+        View o = bufs[(ci + 1) % 4]; o.B = B; o.F = Fs[i]; o.T = Ts[i]; o.C = co; o.ld = co;
+        if (!res2_conv3x3(b, p + ".0", cur, nullptr, o, w, h, WS_ACT_NONE, 2, lvl, kGeminiStrideT[i - 1])) return false;
+        ci = (ci + 1) % 4;
+        cur = o;
+        for (int j = 0; j < e.num_blocks[i - 1]; ++j) {
+            View nx = gemini_block(b, "stages." + std::to_string(i - 1) + "." + std::to_string(j), cur, bufs[(ci + 1) % 4], bufs[(ci + 2) % 4],
+                                   bufs[(ci + 3) % 4], lvl);
+            if (!b.good() || nx.p == nullptr) return false;
+            ci = (ci + 3) % 4;
+            cur = nx;
+        }
+    }
+    return resnet_tail(b, cur, E, 1);
 }
 
 // ----------------------------------------------------------------------------------------------- XVEC
@@ -1697,6 +1823,7 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
         else if (e->model.rfind("ResNet", 0) == 0) ok = build_resnet(b);
         else if (e->model == "XVEC") ok = build_xvec(b);
         else if (e->model.rfind("SimAM_ResNet", 0) == 0) ok = build_simam_resnet(b);
+        else if (e->model.rfind("Gemini_DF_ResNet", 0) == 0) ok = build_gemini(b);
         else if (e->r2_m != 0) {
             Res2Cfg c;
             c.m = e->r2_m; c.base_width = e->r2_base_width; c.scale = e->r2_scale; c.expansion = e->r2_expansion; c.fuse = e->r2_fuse;
@@ -1870,6 +1997,10 @@ static int configure_engine(ws_engine* e, const char* model_name, const char* pr
     else if (m == "CAMPPlus") {}
     else if (m == "SimAM_ResNet34_ASP") e->num_blocks = {3, 4, 6, 3};
     else if (m == "SimAM_ResNet100_ASP") e->num_blocks = {6, 16, 24, 3};
+    else if (m == "Gemini_DF_ResNet60") e->num_blocks = {3, 3, 9, 3};
+    else if (m == "Gemini_DF_ResNet114") e->num_blocks = {3, 3, 27, 3};
+    else if (m == "Gemini_DF_ResNet183") e->num_blocks = {3, 8, 45, 3};
+    else if (m == "Gemini_DF_ResNet237") e->num_blocks = {3, 8, 63, 3};
     else { set_err("unknown / out-of-scope model name: " + m); return 1; }
     const std::string p = e->prec;
     if (p == "fp32") { e->act_dt = WS_F32; e->use_tc = 0; }

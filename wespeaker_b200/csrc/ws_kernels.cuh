@@ -47,6 +47,11 @@ struct WsMapStrides {
 const char* ws_launch_simam_apply(const void* y, long long y_ld, const float* stats, float lambda_p, const void* res, WsMapStrides rs,
                                   void* out, float* out_lo, WsMapStrides os, int dt, int B, int F, int T, int C, cudaStream_t s,
                                   const int* lens = nullptr);
+// Depthwise 3x3 pad-1 conv + folded BN + ReLU (ws_dwconv.cu, gemini_dfresnet.py:37-44): out = relu(dwconv(x, w) + shift) with
+// w fp32 [C][3][3], shift fp32 [C]; rows t >= lens[b] are read as zeros and written as zeros; out_lo (fp32 activations,
+// optional) receives the 3xTF32 low part.  C % 8 == 0 in 16-bit, C % 4 == 0 in fp32.
+const char* ws_launch_dwconv3x3(const void* x, long long x_ld, const float* w, const float* shift, void* out, float* out_lo,
+                                long long out_ld, int dt, int B, int F, int T, int C, cudaStream_t s, const int* lens = nullptr);
 // out[pos][c] = relu(x[pos][c]*scale[c] + shift[c])  (CAM++ pre-activation BN-ReLU, campplus.py:164-166,214)
 const char* ws_launch_bnrelu(const void* x, long long x_ld, const float* scale, const float* shift, void* out,
                              float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s);

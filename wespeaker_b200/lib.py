@@ -45,6 +45,15 @@ class SimamDesc(C.Structure):
     ]
 
 
+class DwConvDesc(C.Structure):
+    """ws_dwconv_desc (include/wespeaker_b200.h)."""
+    _fields_ = [
+        ("x", C.c_void_p), ("x_ld", C.c_longlong), ("B", C.c_int), ("F", C.c_int), ("T", C.c_int), ("C", C.c_int),
+        ("lens", C.c_void_p), ("w", C.c_void_p), ("shift", C.c_void_p), ("out", C.c_void_p), ("out_ld", C.c_longlong),
+        ("out_lo", C.c_void_p), ("dtype", C.c_int),
+    ]
+
+
 _PROTOS = {
     "ws_version": (C.c_int, []),
     "ws_last_error": (C.c_char_p, []),
@@ -86,6 +95,7 @@ _PROTOS = {
                            C.c_void_p]),
     "ws_conv": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     "ws_simam": (C.c_int, [C.POINTER(SimamDesc), C.c_void_p]),
+    "ws_dwconv": (C.c_int, [C.POINTER(DwConvDesc), C.c_void_p]),
     "ws_plda_create": (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                  C.POINTER(c_plda_p)]),
     "ws_plda_transform": (C.c_int, [c_plda_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -20,12 +20,12 @@ import numpy as np
 import torch
 
 from . import lib as _lib
-from .synthetic import (CAMPP_NAMES, DEFAULT_MODEL_ARGS, ECAPA_NAMES, RES2NET_NAMES, RESNET_NAMES, SIMAM_NAMES, XVEC_NAMES,
-                        state_dict_spec)
+from .synthetic import (CAMPP_NAMES, DEFAULT_MODEL_ARGS, ECAPA_NAMES, GEMINI_NAMES, RES2NET_NAMES, RESNET_NAMES, SIMAM_NAMES,
+                        XVEC_NAMES, state_dict_spec)
 
 _IncompatibleKeys = namedtuple("IncompatibleKeys", ["missing_keys", "unexpected_keys"])
 SUPPORTED_MODELS = tuple(ECAPA_NAMES) + tuple(RESNET_NAMES) + tuple(CAMPP_NAMES) + tuple(XVEC_NAMES) + tuple(RES2NET_NAMES) \
-    + tuple(SIMAM_NAMES)
+    + tuple(SIMAM_NAMES) + tuple(GEMINI_NAMES)
 
 
 class B200SpeakerModel(torch.nn.Module):
@@ -225,7 +225,8 @@ class B200SpeakerModel(torch.nn.Module):
         emb = self.embed(features)
         if self.model_name in CAMPP_NAMES or self.model_name in RES2NET_NAMES or self.model_name in SIMAM_NAMES:
             return emb  # campplus.py:409-413, res2net.py:199, eres2net.py:391, samresnet.py:142-149 return a bare tensor
-        # ecapa_tdnn.py:234 returns (out4, emb); resnet.py:204 returns (tensor(0.), embed_a).  Callers use [-1].
+        # ecapa_tdnn.py:234 returns (out4, emb); resnet.py:204 and gemini_dfresnet.py:130-136 return (tensor(0.), embed_a).
+        # Callers use [-1].
         return torch.tensor(0.0), emb
 
     def extract_from_wav(self, wav: torch.Tensor, window_type: str = "hamming", return_feats: bool = False):

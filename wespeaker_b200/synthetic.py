@@ -49,6 +49,10 @@ RES2NET_NAMES = {
 }
 # SimAM-ResNet with ASP pooling, the VoxBlink2 models (`wespeaker/models/samresnet.py:126-167`): block counts
 SIMAM_NAMES = {"SimAM_ResNet34_ASP": [3, 4, 6, 3], "SimAM_ResNet100_ASP": [6, 16, 24, 3]}
+# Gemini DF-ResNet (`wespeaker/models/gemini_dfresnet.py:142-176`): inverted bottlenecks per stage
+GEMINI_NAMES = {"Gemini_DF_ResNet60": [3, 3, 9, 3], "Gemini_DF_ResNet114": [3, 3, 27, 3],
+                "Gemini_DF_ResNet183": [3, 8, 45, 3], "Gemini_DF_ResNet237": [3, 8, 63, 3]}
+GEMINI_DIMS = (32, 32, 64, 128, 256)
 
 DEFAULT_MODEL_ARGS = {
     # examples/voxceleb/v2/conf/{ecapa_tdnn,resnet,campplus}.yaml
@@ -74,6 +78,11 @@ DEFAULT_MODEL_ARGS = {
     # the reference constructor's own arguments (samresnet.py:135): no feat_dim, the feature dimension is acoustic_dim
     "SimAM_ResNet34_ASP": dict(in_planes=64, embed_dim=256, acoustic_dim=80, dropout=0),
     "SimAM_ResNet100_ASP": dict(in_planes=64, embed_dim=256, acoustic_dim=80, dropout=0),
+    # examples/voxceleb/v2/conf/gemini_dfresnet_adam.yaml
+    "Gemini_DF_ResNet60": dict(feat_dim=80, embed_dim=256, pooling_func="TSTP", two_emb_layer=False),
+    "Gemini_DF_ResNet114": dict(feat_dim=80, embed_dim=256, pooling_func="TSTP", two_emb_layer=False),
+    "Gemini_DF_ResNet183": dict(feat_dim=80, embed_dim=256, pooling_func="TSTP", two_emb_layer=False),
+    "Gemini_DF_ResNet237": dict(feat_dim=80, embed_dim=256, pooling_func="TSTP", two_emb_layer=False),
 }
 
 
@@ -337,6 +346,38 @@ def simam_spec(num_blocks, in_planes=64, embed_dim=256, acoustic_dim=80, dropout
     return s
 
 
+def gemini_spec(depths, feat_dim=80, embed_dim=256, pooling_func="TSTP", two_emb_layer=False):
+    """`wespeaker/models/gemini_dfresnet.py:30-136`: ``downsample_layers`` (the stem conv/BN, then four 3x3 convs + BN), the
+    ``stages`` of Inverted_Bottleneck blocks (conv1/bn1 1x1 dim -> 4 dim, conv2/bn2 depthwise 3x3, conv3/bn3 1x1 4 dim -> dim),
+    TSTP over stats_dim = int(feat_dim / 8 / 2) * 256 and the segment layer(s)."""
+    assert pooling_func == "TSTP", "only TSTP is on the hot path for Gemini DF-ResNet"
+    dims = GEMINI_DIMS
+    s = OrderedDict()
+    s["downsample_layers.0.0.weight"] = (dims[0], 1, 3, 3)
+    _bn(s, "downsample_layers.0.1", dims[0])
+    for i in range(4):
+        s[f"downsample_layers.{i + 1}.0.weight"] = (dims[i + 1], dims[i], 3, 3)
+        _bn(s, f"downsample_layers.{i + 1}.1", dims[i + 1])
+    for i, n in enumerate(depths):
+        d = dims[i + 1]
+        for j in range(n):
+            p = f"stages.{i}.{j}"
+            s[f"{p}.conv1.weight"] = (4 * d, d, 1, 1)
+            _bn(s, f"{p}.bn1", 4 * d)
+            s[f"{p}.conv2.weight"] = (4 * d, 1, 3, 3)
+            _bn(s, f"{p}.bn2", 4 * d)
+            s[f"{p}.conv3.weight"] = (d, 4 * d, 1, 1)
+            _bn(s, f"{p}.bn3", d)
+    stats_dim = int(feat_dim / 8 / 2) * dims[-1]
+    s["seg_1.weight"] = (embed_dim, stats_dim * 2)
+    s["seg_1.bias"] = (embed_dim,)
+    if two_emb_layer:
+        _bn(s, "seg_bn_1", embed_dim, affine=False)
+        s["seg_2.weight"] = (embed_dim, embed_dim)
+        s["seg_2.bias"] = (embed_dim,)
+    return s
+
+
 def state_dict_spec(model_name: str, **model_args):
     """key -> shape for a reference model name (`wespeaker/models/speaker_model.py:31-62`)."""
     if model_name in ECAPA_NAMES:
@@ -351,11 +392,19 @@ def state_dict_spec(model_name: str, **model_args):
         return campplus_spec(**model_args)
     if model_name in SIMAM_NAMES:
         return simam_spec(SIMAM_NAMES[model_name], **model_args)
+    if model_name in GEMINI_NAMES:
+        return gemini_spec(GEMINI_NAMES[model_name], **model_args)
     raise ValueError(f"model {model_name!r} is not on the engine's hot path")
 
 
 def _rng(seed: int, key: str) -> np.random.Generator:
     return np.random.Generator(np.random.PCG64([seed, zlib.crc32(key.encode())]))
+
+
+def _gemini_downsample_bn(key):
+    """the BN after each 3x3 conv of Gemini DF-ResNet's ``downsample_layers`` (``downsample_layers.<i>.1.*``)"""
+    parts = key.split(".")
+    return parts[0] == "downsample_layers" and parts[2] == "1"
 
 
 def make_state_dict(model_name: str, seed: int = 0, **model_args):
@@ -374,8 +423,9 @@ def make_state_dict(model_name: str, seed: int = 0, **model_args):
             sd[key] = g.uniform(0.5, 1.5, shape).astype(np.float32)
         elif ".bn" in key or "batchnorm" in key or key.startswith("bn") or "shortcut.1" in key \
                 or "seg_bn" in key or "local_att.1." in key or "local_att.4." in key or "downsample.1." in key \
-                or "pooling.attention.2." in key:
-            if (key.endswith(".bn2.weight") or key.endswith(".bn3.weight")) and "layer" in key:
+                or "pooling.attention.2." in key or _gemini_downsample_bn(key):
+            if (key.endswith(".bn2.weight") or key.endswith(".bn3.weight")) and "layer" in key \
+                    or key.startswith("stages.") and key.endswith(".bn3.weight"):
                 # residual-branch output BN of the 2-D BasicBlocks: keep the residual sum O(1)
                 # over 16 blocks (a trained net does; fp16 range matters for config 3)
                 sd[key] = g.uniform(0.2, 0.6, shape).astype(np.float32)
