@@ -14,44 +14,18 @@ namespace ws {
 
 static thread_local std::string g_err;
 void set_err(const std::string& msg) { g_err = msg; }
-static thread_local std::string g_op_label;
-static thread_local double g_op_flops = 0.0;
-static thread_local bool g_op_has = false;
-void set_op_label(const std::string& name, double flops) { g_op_label = name; g_op_flops = flops; g_op_has = true; }
-bool take_op_label(std::string* name, double* flops) {
-    if (!g_op_has) return false;
-    *name = g_op_label; *flops = g_op_flops; g_op_has = false;
-    return true;
-}
 const std::string& get_err() { return g_err; }
 
 static thread_local bool g_plan_check = false;
 bool plan_check_mode() { return g_plan_check; }
 PlanCheckScope::PlanCheckScope(bool on) : prev(g_plan_check) { g_plan_check = on; }
 PlanCheckScope::~PlanCheckScope() { g_plan_check = prev; }
-static thread_local std::string g_op_trace;
-static thread_local bool g_op_trace_has = false;
-void set_op_trace(const std::string& json) {
-    if (!g_plan_check) return;
-    g_op_trace = json; g_op_trace_has = true;
-}
-bool take_op_trace(std::string* json) {
-    if (!g_op_trace_has) return false;
-    *json = g_op_trace; g_op_trace_has = false;
-    return true;
-}
-static std::string jp(const void* p) { char b[32]; snprintf(b, sizeof b, "%llu", (unsigned long long)p); return b; }
-static std::string jv(const char* name, long long v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%lld", name, v); return b; }
-static std::string jf(float v) { char b[32]; snprintf(b, sizeof b, "%.9g", (double)v); return b; }
-static std::string view_json(const View& v) {
-    return "{\"p\":" + jp(v.p) + "," + jv("B", v.B) + "," + jv("F", v.F) + "," + jv("T", v.T) + "," + jv("C", v.C) + "," + jv("ld", v.ld) + "}";
-}
 static std::string conv_trace(const ConvSpec& s) {
-    std::string j = "{\"kind\":\"conv\"," + jv("es", ws_esize(s.dt)) + ",\"src\":[";
+    std::string j = "{\"kind\":\"conv\"," + ti("es", ws_esize(s.dt)) + ",\"src\":[";
     for (int i = 0; i < s.nsrc; ++i) {
         const WsSrc& v = s.src[i];
-        j += std::string(i ? "," : "") + "{\"p\":" + jp(v.ptr) + "," + jv("B", v.B) + "," + jv("F", v.F) + "," + jv("T", v.T) + "," + jv("C", v.C) + "," +
-             jv("sB", v.sB) + "," + jv("sF", v.sF) + "," + jv("sT", v.sT) + "}";
+        j += std::string(i ? "," : "") + "{" + tp("p", v.ptr) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," +
+             ti("sB", v.sB) + "," + ti("sF", v.sF) + "," + ti("sT", v.sT) + "}";
     }
     j += "],\"taps\":[";
     for (size_t i = 0; i < s.taps.size(); ++i) {
@@ -60,11 +34,11 @@ static std::string conv_trace(const ConvSpec& s) {
              std::to_string(t.wk) + "," + std::to_string(t.nch) + "]";
     }
     const WsEpi& e = s.epi;
-    j += "],\"W\":" + jp(s.W) + "," + jv("Ktot", s.Ktot) + "," + jv("Cout", s.Cout) + "," + jv("B", s.B) + "," + jv("F", s.F) + "," + jv("T", s.T) +
-         ",\"bias\":" + jp(e.bias) + ",\"rowbias\":" + jp(e.rowbias) + "," + jv("rowbias_ld", e.rowbias_ld) + "," + jv("act1", e.act1) + ",\"scale\":" + jp(e.scale) +
-         ",\"shift\":" + jp(e.shift) + ",\"gate\":" + jp(e.gate) + "," + jv("gate_ld", e.gate_ld) + "," + jv("gate_seg", e.gate_seg) + "," + jv("gate_nseg", e.gate_nseg) + ",\"res\":" + jp(e.res) + "," + jv("res_ld", e.res_ld) + "," + jv("act2", e.act2) + ",\"out\":" + jp(e.out) +
-         "," + jv("out_ld", e.out_ld) + ",\"out2\":" + jp(e.out2) + "," + jv("out2_ld", e.out2_ld) + ",\"add2\":" + jp(e.add2) + "," + jv("add2_ld", e.add2_ld) +
-         ",\"colsum\":" + jp(e.colsum) + "}";
+    j += "]," + tp("W", s.W) + "," + ti("Ktot", s.Ktot) + "," + ti("Cout", s.Cout) + "," + ti("B", s.B) + "," + ti("F", s.F) + "," + ti("T", s.T) +
+         "," + tp("bias", e.bias) + "," + tp("rowbias", e.rowbias) + "," + ti("rowbias_ld", e.rowbias_ld) + "," + ti("act1", e.act1) + "," + tp("scale", e.scale) +
+         "," + tp("shift", e.shift) + "," + tp("gate", e.gate) + "," + ti("gate_ld", e.gate_ld) + "," + ti("gate_seg", e.gate_seg) + "," + ti("gate_nseg", e.gate_nseg) + "," + tp("res", e.res) + "," + ti("res_ld", e.res_ld) + "," + ti("act2", e.act2) + "," + tp("out", e.out) +
+         "," + ti("out_ld", e.out_ld) + "," + tp("out2", e.out2) + "," + ti("out2_ld", e.out2_ld) + "," + tp("add2", e.add2) + "," + ti("add2_ld", e.add2_ld) +
+         "," + tp("colsum", e.colsum) + "}";
     return j;
 }
 
@@ -420,14 +394,15 @@ static bool build_simt(const ConvSpec& s, WsSimtParams* p) {
     return true;
 }
 
-static void label_conv(const char* kern, const ConvSpec& spec) {
+static void label_conv(PlanOp* op, const char* kern, const ConvSpec& spec) {
     const double pos = (double)spec.B * spec.F * spec.T;
     char buf[160];
     snprintf(buf, sizeof buf, "%s pos=%lld K=%d N=%d", kern, (long long)pos, spec.Ktot, spec.Cout);
-    set_op_label(buf, 2.0 * pos * spec.Ktot * spec.Cout);
+    op->label = buf;
+    op->flops = 2.0 * pos * spec.Ktot * spec.Cout;
 }
-bool make_conv_op(const ConvSpec& spec, int use_tc, Op* out) {
-    if (plan_check_mode()) set_op_trace(conv_trace(spec));
+bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
+    if (plan_check_mode()) out->trace = conv_trace(spec);
     const char* env_mp = getenv("WS_TC3_MIN_POS");
     const long long min_pos = env_mp ? atoll(env_mp) : 132LL * 128;   // one wave of 128-row tiles on an H100
     if (use_tc >= 3 && (long long)spec.B * spec.F * spec.T >= min_pos) {
@@ -438,12 +413,10 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, Op* out) {
         static const int cl_env = getenv("WS_TC3_CL") ? atoi(getenv("WS_TC3_CL")) : 2;
         const int cl = (cl_env == 4 && (long long)spec.B * spec.F * spec.T >= 2LL * min_pos) ? 4 : 2;
         if (build_tc2(spec, q.get(), &unsupported, cl)) {
-            *out = [q](cudaStream_t s) { return ws_tc3_launch(q.get(), s); };
-            {
-                char kn[64];
-                snprintf(kn, sizeof kn, "conv_tc3 cl=%d grid=%d bn=%d st=%d", q->cl, q->grid, q->bn, q->nstages);
-                label_conv(kn, spec);
-            }
+            out->run = [q](cudaStream_t s) { return ws_tc3_launch(q.get(), s); };
+            char kn[64];
+            snprintf(kn, sizeof kn, "conv_tc3 cl=%d grid=%d bn=%d st=%d", q->cl, q->grid, q->bn, q->nstages);
+            label_conv(out, kn, spec);
             return true;
         }
         if (!unsupported) return false;
@@ -452,8 +425,8 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, Op* out) {
         auto q = std::make_shared<WsTc2Params>();
         bool unsupported = false;
         if (build_tc2(spec, q.get(), &unsupported)) {
-            *out = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
-            label_conv("conv_tc2", spec);
+            out->run = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
+            label_conv(out, "conv_tc2", spec);
             return true;
         }
         if (!unsupported) return false;
@@ -462,19 +435,19 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, Op* out) {
     if (use_tc) {
         auto p = std::make_shared<WsTcParams>();
         if (!build_tc(spec, p.get())) return false;
-        *out = [p](cudaStream_t s) { return ws_tc_launch(p.get(), s); };
-        label_conv("conv_tc1", spec);
+        out->run = [p](cudaStream_t s) { return ws_tc_launch(p.get(), s); };
+        label_conv(out, "conv_tc1", spec);
     } else {
         auto p = std::make_shared<WsSimtParams>();
         if (!build_simt(spec, p.get())) return false;
-        *out = [p](cudaStream_t s) { return ws_simt_launch(p.get(), s); };
-        label_conv("conv_simt", spec);
+        out->run = [p](cudaStream_t s) { return ws_simt_launch(p.get(), s); };
+        label_conv(out, "conv_simt", spec);
     }
     return true;
 }
 
 bool make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
-                  const float* shift, int w8, int dil, Op* op, bool* unsupported, const int* lens) {
+                  const float* shift, int w8, int dil, PlanOp* op, bool* unsupported, const int* lens) {
     *unsupported = false;
     // T > 256: time tiles with a 32-row halo per side cover the chain's receptive field (7 * dil rows) up to dilation 4
     if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7 || getenv("WS_NO_RES2_FUSED")) {
@@ -509,19 +482,18 @@ bool make_res2_op(const View& x, const View& out, const void* W7, const float* b
     q->smem_bytes = npan * 272 * 128 + 4 * w8 * 128 + npan * 256 * 128 + 1024;
     const long long units = (long long)x.B * q->ntile;
     q->grid = (int)(units < ws_num_sms() ? units : ws_num_sms());
-    *op = [q](cudaStream_t s) { return ws_res2_launch(q.get(), s); };
+    op->run = [q](cudaStream_t s) { return ws_res2_launch(q.get(), s); };
     if (plan_check_mode())
-        set_op_trace("{\"kind\":\"res2_fused\",\"es\":2,\"x\":" + view_json(x) + ",\"out\":" + view_json(out) + ",\"W7\":" + jp(W7) + ",\"bias\":" + jp(bias) +
-                     ",\"scale\":" + jp(scale) + ",\"shift\":" + jp(shift) + "," + jv("w8", w8) + "," + jv("dil", dil) + ",\"lens\":" + jp(lens) + "}");
-    {
-        char buf[160];
-        snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", x.B, x.T, x.C);
-        set_op_label(buf, 2.0 * x.B * x.T * 7.0 * 3.0 * (x.C / 8.0) * (x.C / 8.0));
-    }
+        op->trace = "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W7", W7) + "," + tp("bias", bias) +
+                    "," + tp("scale", scale) + "," + tp("shift", shift) + "," + ti("w8", w8) + "," + ti("dil", dil) + "," + tp("lens", lens) + "}";
+    char buf[160];
+    snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", x.B, x.T, x.C);
+    op->label = buf;
+    op->flops = 2.0 * x.B * x.T * 7.0 * 3.0 * (x.C / 8.0) * (x.C / 8.0);
     return true;
 }
 
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, Op* op, bool* unsupported,
+bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, bool* unsupported,
                   const int* lens) {
     *unsupported = false;
     if (x.dt == WS_F32 || h.dt != x.dt || x.C % 128 != 0 || h.C != 128 || h.ld != 128 || x.F != 1 || h.F != 1 || h.T != x.T ||
@@ -570,7 +542,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
         long long* prof = nullptr;
         if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("astp: prof buffer"); return false; }
         q->prof = prof;
-        *op = [q](cudaStream_t s) -> const char* {
+        op->run = [q](cudaStream_t s) -> const char* {
             cudaMemsetAsync(q->prof, 0, (size_t)q->grid * 16 * 8, s);
             const char* m = ws_astp_launch(q.get(), s);
             if (m) return m;
@@ -588,23 +560,22 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
             fprintf(stderr, "\n");
             return nullptr;
         };
-        set_op_label("astp_fused (profiled)", 0.0);
+        op->label = "astp_fused (profiled)";
         return true;
     }
-    *op = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
+    op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
     if (plan_check_mode())
-        set_op_trace("{\"kind\":\"astp_fused\",\"es\":2,\"x\":" + view_json(x) + ",\"h\":" + view_json(h) + ",\"W2\":" + jp(W2) + ",\"stats\":" + jp(stats) +
-                     ",\"lens\":" + jp(lens) + ",\"eps\":" + jf(var_floor) + "}");
-    {
-        char buf[160];
-        snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);
-        set_op_label(buf, 2.0 * x.B * x.T * 128.0 * x.C);
-    }
+        op->trace = "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) +
+                    "," + tp("lens", lens) + "," + tf("eps", var_floor) + "}";
+    char buf[160];
+    snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);
+    op->label = buf;
+    op->flops = 2.0 * x.B * x.T * 128.0 * x.C;
     return true;
 }
 
 bool make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
-                     Op* op, bool* unsupported, int stride_f, int stride_t, const int* lens) {
+                     PlanOp* op, bool* unsupported, int stride_f, int stride_t, const int* lens) {
     *unsupported = false;
     const int Cin = x.C, Cout = out.C, Tin = x.T, Fin = x.F, B = x.B;
     const int F = (Fin + 2 - 3) / stride_f + 1, T = (Tin + 2 - 3) / stride_t + 1;   // output extents
@@ -731,12 +702,21 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
     q->relu = relu;   // 0 none, 1 ReLU, 2 Hardtanh(0, 20)
     q->lens = lens;
     if (const char* dbg = getenv("WS_C3_DBG")) q->dbg = atoi(dbg);
+    char buf[200];
+    snprintf(buf, sizeof buf, "conv3x3 B=%d F=%d T=%d Cin=%d Cout=%d s=%dx%d caseB=%d nb=%d n_mt=%d R=%d res=%d", q->B, q->F, q->T,
+             q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
+    op->label = buf;
+    op->flops = 2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout;
+    if (plan_check_mode())
+        op->trace = "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) +
+                    "," + (res ? tview("res", *res) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) +
+                    "," + tp("lens", lens) + "}";
     if (getenv("WS_C3_PROF")) {   // tuning aid: synchronous launch + per-role wait-cycle summary on stderr
         long long* prof = nullptr;
         if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("conv3x3: prof buffer"); return false; }
         cudaMemset(prof, 0, (size_t)q->grid * 16 * 8);
         q->prof = prof;
-        *op = [q](cudaStream_t s) -> const char* {
+        op->run = [q](cudaStream_t s) -> const char* {
             const char* m = ws_c3_launch(q.get(), s);
             if (m) return m;
             cudaStreamSynchronize(s);
@@ -756,17 +736,7 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
         };
         return true;
     }
-    *op = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
-    if (plan_check_mode())
-        set_op_trace("{\"kind\":\"conv3x3\",\"es\":2,\"x\":" + view_json(x) + ",\"out\":" + view_json(out) + ",\"W\":" + jp(W) + ",\"bias\":" + jp(bias) +
-                     ",\"res\":" + (res ? view_json(*res) : std::string("null")) + "," + jv("relu", relu) + "," + jv("sf", stride_f) + "," + jv("st", stride_t) +
-                     ",\"lens\":" + jp(lens) + "}");
-    {
-        char buf[200];
-        snprintf(buf, sizeof buf, "conv3x3 B=%d F=%d T=%d Cin=%d Cout=%d s=%dx%d caseB=%d nb=%d n_mt=%d R=%d res=%d", q->B, q->F, q->T,
-                 q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
-        set_op_label(buf, 2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout);
-    }
+    op->run = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
     return true;
 }
 
@@ -795,7 +765,7 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
     return true;
 }
 
-bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, Op* op, bool* unsupported,
+bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, bool* unsupported,
                        const int* lens) {
     *unsupported = false;
     const int T = X.T, B = X.B;
@@ -819,12 +789,15 @@ bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int 
     cuuint32_t boxx[3] = {64, 128, 1}, boxo[3] = {32, 128, 1};
     if (!encode_map(&q->xmap, X.dt, X.p, 3, dims, str, boxx, 128)) return false;
     if (!encode_map(&q->omap, X.dt, X.p, 3, dims, str, boxo, 64)) return false;
+    char buf[160];
+    snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
+    op->label = buf;
     if (getenv("WS_CAM_PROF")) {   // tuning aid: synchronous launch + phase timestamps (cycles since kernel start) of CTA 0
         long long* prof = nullptr;
         if (cudaMalloc((void**)&prof, 16 * 8) != cudaSuccess) { set_err("cam_dense: prof buffer"); return false; }
         cudaMemset(prof, 0, 16 * 8);
         q->prof = prof;
-        *op = [q](cudaStream_t s) -> const char* {
+        op->run = [q](cudaStream_t s) -> const char* {
             const char* m = ws_cam_launch(q.get(), s);
             if (m) return m;
             cudaStreamSynchronize(s);
@@ -839,12 +812,7 @@ bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int 
         };
         return true;
     }
-    *op = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
-    {
-        char buf[160];
-        snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
-        set_op_label(buf, 0.0);
-    }
+    op->run = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
     return true;
 }
 
@@ -873,7 +841,7 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
     s.epi.bias = d->bias; s.epi.act1 = d->act1; s.epi.scale = d->scale; s.epi.shift = d->shift;
     s.epi.res = d->res; s.epi.res_ld = d->res_ld; s.epi.act2 = d->act2;
     s.epi.colsum = d->colsum; s.epi.colsum_T = d->colsum ? To : 0;
-    Op op;
+    PlanOp op;
     if (d->use_tc) { WS_CKS(ws_tc_init()); WS_CKS(ws_tc2_init()); WS_CKS(ws_tc3_init()); WS_CKS(ws_c3_init()); WS_CKS(ws_astp_init()); }
     bool done = false;
     if (d->use_tc >= 4 && d->kf == 3 && d->kt == 3 && d->dil_f == 1 && d->dil_t == 1 && d->pad_f == 1 && d->pad_t == 1 &&
@@ -890,7 +858,7 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
         else if (!unsupported) return 1;
     }
     if (!done && !make_conv_op(s, d->use_tc >= 4 ? 3 : d->use_tc, &op)) return 1;
-    const char* m = op((cudaStream_t)stream);
+    const char* m = op.run((cudaStream_t)stream);
     if (m != nullptr) { set_err(std::string("ws_conv launch: ") + m); return 1; }
     return 0;
 }

@@ -39,10 +39,7 @@ struct FbankTables {
 
 struct Plan {
     int B = 0, T = 0;
-    std::vector<Op> ops;
-    std::vector<std::string> op_names;   // tuning aid (ws_engine_profile_ops): label and FLOPs per op
-    std::vector<double> op_flops;
-    std::vector<std::string> op_traces;  // plan-check engines: JSON description of each op (ws_engine_plan_trace), else empty strings
+    std::vector<PlanOp> ops;
     std::vector<void*> bufs;
     int extra_launches = 0;     // ops that launch more than one kernel (split-K FC = 2)
     size_t bytes = 0;           // device memory held by this plan
@@ -223,9 +220,9 @@ struct Weights {
         }
         return true;
     }
-    // conv weight (Cout, Cin, k) or (Cout, Cin, kf, kt) -> [Cout][tap][Cin] (tap-major), optional per-row scale
-    bool pack_conv(const std::string& key, const std::vector<float>* rowscale, std::vector<float>& out, int* Cout,
-                   int* Cin, int* ntap) {
+    // conv weight (Cout, Cin, k) or (Cout, Cin, kf, kt) -> [Cout][tap][Cin] (tap-major), optional per-row scale and shape
+    bool pack_conv(const std::string& key, const std::vector<float>* rowscale, std::vector<float>& out, int* Cout = nullptr,
+                   int* Cin = nullptr, int* ntap = nullptr) {
         const HostT* t = get(key);
         if (!t) return false;
         const int co = (int)t->shape[0], ci = (int)t->shape[1];
@@ -238,7 +235,9 @@ struct Weights {
                 for (int j = 0; j < taps; ++j)
                     out[((size_t)o * taps + j) * ci + c] = t->v[((size_t)o * ci + c) * taps + j] * sc;
         }
-        *Cout = co; *Cin = ci; *ntap = taps;
+        if (Cout) *Cout = co;
+        if (Cin) *Cin = ci;
+        if (ntap) *ntap = taps;
         return true;
     }
 };
@@ -274,24 +273,20 @@ struct Builder {
         return v;
     }
     float* f32(size_t n) { return (float*)raw(n * 4); }
-    void push(Op op, const char* name = nullptr) {
-        std::string label;
-        double flops = 0.0;
-        const bool had = take_op_label(&label, &flops);
-        if (name) { label = name; if (!had) flops = 0.0; }
-        else if (!had) label = "op";
-        p.ops.push_back(std::move(op));
-        p.op_names.push_back(label);
-        p.op_flops.push_back(flops);
-        std::string tr;
-        take_op_trace(&tr);
-        p.op_traces.push_back(tr);
+    // n rotating activation buffers of `elems` elements each (with their 3xTF32 lo twins)
+    std::vector<View> ring(int n, size_t elems) {
+        std::vector<View> v((size_t)n);
+        for (View& x : v) {
+            x.dt = e.act_dt;
+            x.p = raw(elems * ws_esize(e.act_dt));
+            if (e.split) x.plo = raw(elems * 4);
+        }
+        return v;
     }
-    // plan-trace helpers (no-ops outside plan-check mode): "name":address / "name":integer fields of an op description
-    static std::string tp(const char* n, const void* q) { char bf[96]; snprintf(bf, sizeof bf, "\"%s\":%llu", n, (unsigned long long)q); return bf; }
-    static std::string ti(const char* n, long long v) { char bf[96]; snprintf(bf, sizeof bf, "\"%s\":%lld", n, v); return bf; }
-    static std::string tview(const char* n, const View& v) {
-        return std::string("\"") + n + "\":{" + tp("p", v.p) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
+    void push(PlanOp op) { p.ops.push_back(std::move(op)); }
+    // a bandwidth op: launch closure, label, and its plan-trace description (kept in plan-check mode only)
+    void push(Op run, const char* label, std::string trace) {
+        push(PlanOp{std::move(run), label, 0.0, plan_check_mode() ? std::move(trace) : std::string()});
     }
     // length-masked plans: frame counts of stride level k (nullptr in ordinary plans), and "zero the rows behind every
     // utterance's end" for tensors a time-mixing op is about to read (the reference's unpadded forward sees zero padding)
@@ -300,8 +295,8 @@ struct Builder {
         if (!p.masked) return;
         const View x = v;
         const int* l = lens(level);
-        set_op_trace("{\"kind\":\"zero_tail\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("lens", l) + "}");
-        push([=](cudaStream_t s) { return ws_launch_zero_tail(x.p, (float*)x.plo, x.dt, x.B, x.F, x.T, x.C, x.ld, l, s); }, "zero_tail");
+        push([=](cudaStream_t s) { return ws_launch_zero_tail(x.p, (float*)x.plo, x.dt, x.B, x.F, x.T, x.C, x.ld, l, s); }, "zero_tail",
+             "{\"kind\":\"zero_tail\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("lens", l) + "}");
     }
     void conv(const ConvSpec& s_in) {
         if (!good()) return;
@@ -312,7 +307,7 @@ struct Builder {
             s.W_lo = it->second;
             s.split = true;
         }
-        Op op;
+        PlanOp op;
         if (!make_conv_op(s, e.use_tc, &op)) { ok = false; return; }
         push(std::move(op));
     }
@@ -341,12 +336,11 @@ struct Builder {
                 int level = 0) {
         View xv = x;
         const int* l = lens(level);
-        set_op_trace("{\"kind\":\"tstats\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("pre_scale", pre_scale) + "," + tp("pre_shift", pre_shift) + "," +
-                     tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("std_off", std_off) + "," + tp("lens", l) + "}");
         push([=](cudaStream_t s) {
             return ws_launch_tstats(xv.p, xv.dt, xv.B, xv.F, xv.T, xv.C, xv.ld, pre_scale, pre_shift, out, WS_F32, out_ld,
                                     std_off, 1e-7f, s, l);
-        }, "tstats");
+        }, "tstats", "{\"kind\":\"tstats\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("pre_scale", pre_scale) + "," + tp("pre_shift", pre_shift) + "," +
+                     tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("std_off", std_off) + "," + tp("lens", l) + "}");
     }
     void linear(const float* in, long long in_ld, const float* in2, long long in2_ld, int rows_per_b, const float* W,
                 const float* bias, float* out, long long out_ld, int R, int I, int O, int act) {
@@ -359,12 +353,106 @@ struct Builder {
         else while (blocks * nsplit < 2 * sms && I / (nsplit * 2) >= 128 && nsplit < 16) nsplit *= 2;
         float* wsp = nsplit > 1 ? f32((size_t)nsplit * R * O) : nullptr;
         if (nsplit > 1) p.extra_launches += 1;
-        set_op_trace("{\"kind\":\"linear\"," + tp("in", in) + "," + ti("in_ld", in_ld) + "," + tp("in2", in2) + "," + ti("in2_ld", in2_ld) + "," + ti("rows_per_b", rows_per_b) + "," +
-                     tp("W", W) + "," + tp("bias", bias) + "," + tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("R", R) + "," + ti("I", I) + "," + ti("O", O) + "," + ti("act", act) + "}");
         push([=](cudaStream_t s) {
             return ws_launch_linear_rows(in, in_ld, in2, in2_ld, rows_per_b, W, bias, out, out_ld, R, I, O, act, wsp,
                                          nsplit, s);
-        }, "linear_rows");
+        }, "linear_rows", "{\"kind\":\"linear\"," + tp("in", in) + "," + ti("in_ld", in_ld) + "," + tp("in2", in2) + "," + ti("in2_ld", in2_ld) + "," + ti("rows_per_b", rows_per_b) + "," +
+                     tp("W", W) + "," + tp("bias", bias) + "," + tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("R", R) + "," + ti("I", I) + "," + ti("O", O) + "," + ti("act", act) + "}");
+    }
+    // the fp32 input features -> x0 (B,1,T,feat_dim) in the activation dtype
+    void convert_input(const View& x0) {
+        const float* fin = p.feats_in;
+        void* xo = x0.p;
+        float* xlo = (float*)x0.plo;
+        const int dt = x0.dt;
+        const long long n = x0.npos() * x0.C;
+        push([=](cudaStream_t s) { return ws_launch_convert(fin, xo, xlo, dt, n, s); }, "convert",
+             "{\"kind\":\"convert\"," + ti("es", ws_esize(dt)) + "," + tp("in", fin) + "," + tp("out", xo) + "," + ti("n", n) + "}");
+    }
+    // out = relu(x * scale + shift), per channel over x's C channels
+    void bnrelu(const View& x, const float* scale, const float* shift, const View& out) {
+        const View xv = x, ov = out;
+        const int C = x.C;
+        const long long npos = x.npos();
+        push([=](cudaStream_t s) { return ws_launch_bnrelu(xv.p, xv.ld, scale, shift, ov.p, (float*)ov.plo, ov.ld, xv.dt, npos, C, s); }, "bnrelu",
+             "{\"kind\":\"bnrelu\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("scale", scale) + "," + tp("shift", shift) + "," +
+             tview("out", out) + "," + ti("C", C) + "}");
+    }
+    // The halo-resident 3x3 pad-1 conv (ws_conv3x3.cu: every input row crosses L2 -> SM once instead of once per tap),
+    // out = act(conv(x, W) + bias [+ res]).  halo3x3: whether the precision and the options let convs of strides (sf, st) use
+    // it.  halo_conv3x3 returns 1 with *op built (not pushed), 0 when the caller runs the conv-GEMM instead (also when the
+    // shape is outside the kernel's envelope), -1 on error.  lvl: stride level of `out`.
+    bool halo3x3(int sf, int st) const {
+        return e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("conv3x3", 1) != 0 && ((sf == 1 && st == 1) || e.opt("conv3x3_strided", 1) != 0);
+    }
+    int halo_conv3x3(const View& x, const View& out, const void* W, const float* bias, const View* res, int act, int sf, int st, int lvl,
+                     PlanOp* op) {
+        if (!halo3x3(sf, st)) return 0;
+        bool unsupported = false;
+        if (make_conv3x3_op(x, out, W, bias, res, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, op, &unsupported, sf, st, lens(lvl)))
+            return 1;
+        if (unsupported) return 0;
+        ok = false;
+        return -1;
+    }
+    // 3x3 pad-1 conv, out = act(conv(x, W) + bias), act WS_ACT_RELU20, WS_ACT_RELU or WS_ACT_NONE: the halo-resident kernel where
+    // it applies, else the conv-GEMM, followed (length-masked plans) by zeroing the rows behind every utterance's end unless the
+    // caller's next reader does not mix time (`zero_tail_after` = false)
+    bool conv3x3(const View& x, const View& out, const void* W, const float* bias, int act, int sf, int st, int lvl, bool zero_tail_after = true) {
+        PlanOp op;
+        const int r = halo_conv3x3(x, out, W, bias, nullptr, act, sf, st, lvl, &op);
+        if (r > 0) push(std::move(op));
+        if (r != 0) return good();
+        WsEpi ep{};
+        ep.bias = bias;
+        ep.act1 = act;
+        conv_simple(x, out, W, 3, 3, 1, 1, 1, 1, sf, st, ep);
+        if (zero_tail_after) zero_tail(out, lvl);
+        return good();
+    }
+    // The strided 1x1 shortcut conv `pfx`.shortcut.0 (with its BN `pfx`.shortcut.1 folded in) over x as one more K range of the
+    // block's last conv `cs` (output o): its weights are appended to every row of wk ([o.C][K] -> [o.C][K + x.C]) and its BN
+    // shift is added to bias.
+    bool merge_shortcut(ConvSpec& cs, const std::string& pfx, const View& x, int sf, int st, const View& o, std::vector<float>& wk, int& K,
+                        std::vector<float>& bias) {
+        std::vector<float> ss, hs, wsv;
+        int co = 0;
+        if (!w.bn(pfx + ".shortcut.1", true, ss, hs) || !w.pack_conv(pfx + ".shortcut.0.weight", &ss, wsv, &co)) return false;
+        int Fs, Ts;
+        const int K2 = add_conv_taps(cs, x, 1, 1, 1, 1, 0, 0, sf, st, K, &Fs, &Ts);
+        if (K2 != x.C || co != o.C || (int)wsv.size() != o.C * K2 || Fs != o.F || Ts != o.T) { set_err(pfx + ": shortcut shape mismatch"); ok = false; return false; }
+        std::vector<float> wm((size_t)o.C * (K + K2));
+        for (int r = 0; r < o.C; ++r) {
+            memcpy(&wm[(size_t)r * (K + K2)], &wk[(size_t)r * K], (size_t)K * 4);
+            memcpy(&wm[(size_t)r * (K + K2) + K], &wsv[(size_t)r * K2], (size_t)K2 * 4);
+        }
+        wk.swap(wm);
+        K += K2;
+        for (int i = 0; i < o.C; ++i) bias[i] += hs[i];
+        return true;
+    }
+    // Attentive statistics (pooling_layers.py): logits = W2 h + bias2, softmax over time per channel, stats = [mean | sqrt(max(var,
+    // eps))] of x under those weights.  The fused op where it applies (bias2 cancels in the softmax), else linear2 as a conv plus
+    // astp_stats.  lvl: stride level of x
+    bool astp_tail(const View& x, const View& h, const void* W2, const float* bias2, float* stats, double eps, int lvl) {
+        const int* l = lens(lvl);
+        if (e.use_tc >= 2 && e.opt("astp_fused", 1) && good()) {
+            PlanOp op;
+            bool unsupported = false;
+            if (make_astp_op(x, h, W2, stats, (float)eps, &op, &unsupported, l)) { push(std::move(op)); return true; }
+            if (!unsupported) { ok = false; return false; }
+        }
+        View logits = act(x.B, 1, x.T, x.C);
+        WsEpi ep{};
+        ep.bias = bias2;
+        conv_simple(h, logits, W2, 1, 1, 1, 1, 0, 0, 1, 1, ep);
+        if (!good()) return false;
+        const View fr = x, lg = logits;
+        const float var_floor = (float)eps;
+        push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, fr.B, fr.T, fr.C, fr.ld, stats, var_floor, s, l); }, "astp_stats",
+             "{\"kind\":\"astp_stats\"," + ti("es", ws_esize(fr.dt)) + "," + tview("x", fr) + "," + tview("logits", lg) + "," + tp("stats", stats) + "," +
+             tp("lens", l) + "," + tf("eps", eps) + "}");
+        return good();
     }
 };
 
@@ -384,21 +472,12 @@ bool build_ecapa(Builder& b) {
     float* segate = b.f32((size_t)B * C);
     float* stats = b.f32((size_t)B * 3072);
     if (!b.good()) return false;
-    {
-        const float* fin = b.p.feats_in;
-        void* xo = x0.p;
-        float* xlo = (float*)x0.plo;
-        const int dt = e.act_dt;
-        const long long n = (long long)B * T * Fd;
-        set_op_trace("{\"kind\":\"convert\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tp("in", fin) + "," + Builder::tp("out", xo) + "," + Builder::ti("n", n) + "}");
-        b.push([=](cudaStream_t s) { return ws_launch_convert(fin, xo, xlo, dt, n, s); }, "convert");
-        b.zero_tail(x0, 0);   // (masked plans) the k=5 conv of layer1 must see zero padding behind each utterance
-    }
+    b.convert_input(x0);
+    b.zero_tail(x0, 0);   // (masked plans) the k=5 conv of layer1 must see zero padding behind each utterance
     // Conv1dReluBn (ecapa_tdnn.py:85-106): bn(relu(conv(x)+bias))
     auto conv_relu_bn = [&](const std::string& pfx, const View& x, const View& out, int k, int dil, int pad) {
         std::vector<float> wp, s, h;
-        int co, ci, nt;
-        if (!b.w.pack_conv(pfx + ".conv.weight", nullptr, wp, &co, &ci, &nt) || !b.w.bn(pfx + ".bn", true, s, h)) return;
+        if (!b.w.pack_conv(pfx + ".conv.weight", nullptr, wp) || !b.w.bn(pfx + ".bn", true, s, h)) return;
         WsEpi ep{};
         ep.bias = b.w.vec(pfx + ".conv.bias");
         ep.act1 = WS_ACT_RELU;
@@ -426,9 +505,8 @@ bool build_ecapa(Builder& b) {
             for (int i = 0; i < 7 && okw; ++i) {
                 const std::string cp = pf + ".1.convs." + std::to_string(i), bp = pf + ".1.bns." + std::to_string(i);
                 std::vector<float> wp, s, h;
-                int co, ci, nt;
                 const HostT* bt = b.w.get(cp + ".bias");
-                okw = bt && b.w.pack_conv(cp + ".weight", nullptr, wp, &co, &ci, &nt) && b.w.bn(bp, true, s, h);
+                okw = bt && b.w.pack_conv(cp + ".weight", nullptr, wp) && b.w.bn(bp, true, s, h);
                 if (!okw) break;
                 memcpy(&w7[(size_t)i * w8 * 3 * w8], wp.data(), wp.size() * 4);
                 memcpy(&b7[(size_t)i * w8], bt->v.data(), (size_t)w8 * 4);
@@ -436,7 +514,7 @@ bool build_ecapa(Builder& b) {
                 memcpy(&h7[(size_t)i * w8], h.data(), (size_t)w8 * 4);
             }
             if (!okw) break;
-            Op op;
+            PlanOp op;
             bool unsupported = false;
             if (make_res2_op(tA, tB, b.w.act("w7:" + pf, w7), b.w.f32("b7:" + pf, b7), b.w.f32("s7:" + pf, s7),
                              b.w.f32("h7:" + pf, h7), w8, d, &op, &unsupported, b.lens(0))) {
@@ -450,8 +528,7 @@ bool build_ecapa(Builder& b) {
         for (int i = 0; i < 7 && b.good() && !fused; ++i) {
             const std::string cp = pf + ".1.convs." + std::to_string(i), bp = pf + ".1.bns." + std::to_string(i);
             std::vector<float> wp, s, h;
-            int co, ci, nt;
-            if (!b.w.pack_conv(cp + ".weight", nullptr, wp, &co, &ci, &nt) || !b.w.bn(bp, true, s, h)) break;
+            if (!b.w.pack_conv(cp + ".weight", nullptr, wp) || !b.w.bn(bp, true, s, h)) break;
             WsEpi ep{};
             ep.bias = b.w.vec(cp + ".bias");
             ep.act1 = WS_ACT_RELU;
@@ -470,8 +547,7 @@ bool build_ecapa(Builder& b) {
         {   // third block: 1x1 conv over cat[sp_0..sp_6, spx_7]: two K ranges from two buffers
             const std::string cp = pf + ".2";
             std::vector<float> wp, s, h;
-            int co, ci, nt;
-            if (!b.w.pack_conv(cp + ".conv.weight", nullptr, wp, &co, &ci, &nt) || !b.w.bn(cp + ".bn", true, s, h)) break;
+            if (!b.w.pack_conv(cp + ".conv.weight", nullptr, wp) || !b.w.bn(cp + ".bn", true, s, h)) break;
             ConvSpec cs;
             cs.dt = e.act_dt;
             cs.src[0] = Builder::src_of(tB.ch(0, 7 * w8));
@@ -506,9 +582,9 @@ bool build_ecapa(Builder& b) {
             const int dt = e.act_dt;
             const float* cs_in = se_colsum;
             const int* l0 = b.lens(0);
-            set_op_trace("{\"kind\":\"se_gate\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", tc) + "," + Builder::tp("W1", w1d) + "," + Builder::tp("b1", b1d) + "," +
-                         Builder::tp("W2t", w2d) + "," + Builder::tp("b2", b2d) + "," + Builder::ti("H", 128) + "," + Builder::tp("gate", segate) + "," + Builder::tp("lens", l0) + "}");
-            b.push([=](cudaStream_t s) { return ws_launch_se_gate(tc.p, dt, B, T, C, tc.ld, w1d, b1d, w2d, b2d, 128, segate, cs_in, s, l0); }, "se_gate");
+            b.push([=](cudaStream_t s) { return ws_launch_se_gate(tc.p, dt, B, T, C, tc.ld, w1d, b1d, w2d, b2d, 128, segate, cs_in, s, l0); }, "se_gate",
+                   "{\"kind\":\"se_gate\"," + ti("es", ws_esize(dt)) + "," + tview("x", tc) + "," + tp("W1", w1d) + "," + tp("b1", b1d) + "," +
+                   tp("W2t", w2d) + "," + tp("b2", b2d) + "," + ti("H", 128) + "," + tp("gate", segate) + "," + tp("lens", l0) + "}");
         } else {
             b.tstats(tC, nullptr, nullptr, semean, C, -1);
             b.linear(semean, C, nullptr, 0, 1, b.w.vec(pf + ".3.linear1.weight"), b.w.vec(pf + ".3.linear1.bias"), sehid, 128, B,
@@ -519,19 +595,17 @@ bool build_ecapa(Builder& b) {
         {
             View o = cat.ch((L - 2) * C, C), xi = xin, tc = tC;
             const int dt = e.act_dt;
-            set_op_trace("{\"kind\":\"scale_residual\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", tc) + "," + Builder::tp("gate", segate) + "," +
-                         Builder::tview("res", xi) + "," + Builder::tview("out", o) + "}");
             b.push([=](cudaStream_t s) {
                 return ws_launch_scale_residual(tc.p, tc.ld, segate, xi.p, xi.ld, o.p, (float*)o.plo, o.ld, dt, B, T, C, s);
-            }, "scale_residual");
+            }, "scale_residual", "{\"kind\":\"scale_residual\"," + ti("es", ws_esize(dt)) + "," + tview("x", tc) + "," + tp("gate", segate) + "," +
+                                 tview("res", xi) + "," + tview("out", o) + "}");
             xin = o;
         }
     }
     if (!b.good()) return false;
     {   // self.conv (1x1, 3C -> 1536) then F.relu (ecapa_tdnn.py:217-218,229)
         std::vector<float> wp;
-        int co, ci, nt;
-        if (!b.w.pack_conv("conv.weight", nullptr, wp, &co, &ci, &nt)) return false;
+        if (!b.w.pack_conv("conv.weight", nullptr, wp)) return false;
         WsEpi ep{};
         ep.bias = b.w.vec("conv.bias");
         ep.act1 = WS_ACT_RELU;
@@ -566,28 +640,10 @@ bool build_ecapa(Builder& b) {
         ep.act1 = WS_ACT_TANH;
         b.conv_simple(frame, hid, b.w.act("w:pool.linear1.x", wx), 1, 1, 1, 1, 0, 0, 1, 1, ep);
         std::vector<float> w2;
-        int co, ci, nt;
-        if (!b.w.pack_conv("pool.linear2.weight", nullptr, w2, &co, &ci, &nt)) return false;
-        const void* W2d = b.w.act("w:pool.linear2", w2);
-        const int* l0 = b.lens(0);
-        // linear2 + softmax over time + weighted statistics in one launch: the logits never leave the SM (ws_astp_fused.cu)
-        bool fused = false;
-        if (e.use_tc >= 2 && e.opt("astp_fused", 1) && b.good()) {
-            Op op;
-            bool unsupported = false;
-            if (make_astp_op(frame, hid, W2d, stats, 1e-7f, &op, &unsupported, l0)) { b.push(std::move(op)); fused = true; }
-            else if (!unsupported) { b.ok = false; return false; }
-        }
-        if (!fused) {
-            View logits = b.act(B, 1, T, 1536);
-            WsEpi ep2{};
-            ep2.bias = b.w.vec("pool.linear2.bias");
-            b.conv_simple(hid, logits, W2d, 1, 1, 1, 1, 0, 0, 1, 1, ep2);
-            View fr = frame, lg = logits;
-            set_op_trace("{\"kind\":\"astp_stats\"," + Builder::ti("es", ws_esize(fr.dt)) + "," + Builder::tview("x", fr) + "," + Builder::tview("logits", lg) + "," +
-                         Builder::tp("stats", stats) + "," + Builder::tp("lens", l0) + ",\"eps\":1e-07}");
-            b.push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, B, T, 1536, fr.ld, stats, 1e-7f, s, l0); }, "astp_stats");
-        }
+        if (!b.w.pack_conv("pool.linear2.weight", nullptr, w2)) return false;
+        // linear2 + softmax over time + weighted statistics, fused into one launch where it applies: the logits never leave
+        // the SM (ws_astp_fused.cu)
+        if (!b.astp_tail(frame, hid, b.w.act("w:pool.linear2", w2), b.w.vec("pool.linear2.bias"), stats, 1e-7, 0)) return false;
     }
     {   // bn(3072) then linear (ecapa_tdnn.py:230-231): fold the affine into the linear; optional bn2 (emb_bn)
         std::vector<float> s, h;
@@ -618,89 +674,43 @@ bool build_ecapa(Builder& b) {
 // `lvl`: stride level of the block's OUTPUT (length-masked plans: frame counts b.lens(lvl)); the time stride st_ is 1 or 2
 View basic_block(Builder& b, const std::string& p, const View& x, int cout, int sf, int st_, View hbuf, View obuf, int lvl = 0) {
     std::vector<float> s1, h1, s2, h2, w1, w2;
-    int co, ci, nt;
     View none;
-    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) ||
-        !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co, &ci, &nt) || !b.w.pack_conv(p + ".conv2.weight", &s2, w2, &co, &ci, &nt))
+    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1) ||
+        !b.w.pack_conv(p + ".conv2.weight", &s2, w2))
         return none;
     const int Fo = (x.F + 2 - 3) / sf + 1, To = (x.T + 2 - 3) / st_ + 1;
-    View h = hbuf; h.B = x.B; h.F = Fo; h.T = To; h.C = cout; h.ld = cout;
-    View o = obuf; o.B = x.B; o.F = Fo; o.T = To; o.C = cout; o.ld = cout;
-    // stride-1 3x3 convs of the low-channel stages run the halo-resident kernel (ws_conv3x3.cu): every input row crosses
-    // L2 -> SM once instead of once per tap
-    const bool c3 = b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0;
-    auto try_c3 = [&](const View& in, const View& outv, const void* Wd, const float* bias, const View* res, int s_f, int s_t) -> int {
-        if (!c3) return 0;
-        Op op;
-        bool unsupported = false;
-        if (make_conv3x3_op(in, outv, Wd, bias, res, true, &op, &unsupported, s_f, s_t, b.lens(lvl))) { b.push(std::move(op)); return 1; }
-        if (!unsupported) { b.ok = false; return -1; }
-        return 0;
-    };
-    {
-        const float* b1 = b.w.f32("bnh:" + p + ".bn1", h1);
-        const void* W1 = b.w.act("w:" + p + ".conv1", w1);
-        int r = (b.e.opt("conv3x3_strided", 1) != 0 || (sf == 1 && st_ == 1)) ? try_c3(x, h, W1, b1, nullptr, sf, st_) : 0;
-        if (r < 0) return none;
-        if (r == 0) {
-            WsEpi e1{};
-            e1.bias = b1;
-            e1.act1 = WS_ACT_RELU;
-            b.conv_simple(x, h, W1, 3, 3, 1, 1, 1, 1, sf, st_, e1);
-            b.zero_tail(h, lvl);
-        }
-    }
-    if (!b.good()) return none;
-    const bool has_sc0 = b.e.sd.count(p + ".shortcut.0.weight") != 0;
-    if (c3 && (cout == 32 || cout == 64 || cout == 128)) {
+    const View h = hbuf.shaped(x.B, Fo, To, cout), o = obuf.shaped(x.B, Fo, To, cout);
+    if (!b.conv3x3(x, h, b.w.act("w:" + p + ".conv1", w1), b.w.f32("bnh:" + p + ".bn1", h1), WS_ACT_RELU, sf, st_, lvl)) return none;
+    const bool has_sc = b.e.sd.count(p + ".shortcut.0.weight") != 0;
+    if (b.halo3x3(1, 1) && (cout == 32 || cout == 64 || cout == 128)) {
         // conv2 on the halo-resident kernel: the 1x1 strided shortcut conv (+ its BN) is written to `o` first and then
-        // read back as the residual, in place (each output element is read and written by the same CTA step)
-        const float* b2 = b.w.f32("bnh:" + p + ".bn2", h2);
-        const void* W2 = b.w.act("w:" + p + ".conv2", w2);
-        // build conv2's launch first: if the shape is outside the kernel's envelope nothing has been emitted yet
-        View resv = has_sc0 ? o : x;
-        Op op2;
-        bool unsupported = false;
-        if (make_conv3x3_op(h, o, W2, b2, &resv, true, &op2, &unsupported, 1, 1, b.lens(lvl))) {
-            std::string lab2, tr2;
-            double fl2 = 0.0;
-            take_op_label(&lab2, &fl2);
-            const bool had_tr2 = take_op_trace(&tr2);
-            if (has_sc0) {
+        // read back as the residual, in place (each output element is read and written by the same CTA step).  conv2's op is
+        // built first: if the shape is outside the kernel's envelope nothing has been emitted yet.  (The channel counts the
+        // kernel takes are checked here so that other blocks do not upload conv2's unmerged weights.)
+        const View res = has_sc ? o : x;
+        PlanOp op2;
+        const int r = b.halo_conv3x3(h, o, b.w.act("w:" + p + ".conv2", w2), b.w.f32("bnh:" + p + ".bn2", h2), &res, WS_ACT_RELU, 1, 1, lvl, &op2);
+        if (r < 0) return none;
+        if (r > 0) {
+            if (has_sc) {
                 std::vector<float> ss, hs, wsv;
-                if (!b.w.bn(p + ".shortcut.1", true, ss, hs) || !b.w.pack_conv(p + ".shortcut.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
+                if (!b.w.bn(p + ".shortcut.1", true, ss, hs) || !b.w.pack_conv(p + ".shortcut.0.weight", &ss, wsv)) return none;
                 WsEpi es{};
                 es.bias = b.w.f32("bnh:" + p + ".shortcut", hs);
                 b.conv_simple(x, o, b.w.act("w:" + p + ".shortcut", wsv), 1, 1, 1, 1, 0, 0, sf, st_, es);
                 if (!b.good()) return none;
             }
-            set_op_label(lab2, fl2);
-            if (had_tr2) set_op_trace(tr2);
             b.push(std::move(op2));
             return o;
         }
-        if (!unsupported) { b.ok = false; return none; }
     }
     ConvSpec cs;
     cs.dt = b.e.act_dt;
     int F2, T2;
     int K = add_conv_taps(cs, h, 3, 3, 1, 1, 1, 1, 1, 1, 0, &F2, &T2);
     std::vector<float> bias2 = h2;
-    const bool has_sc = b.e.sd.count(p + ".shortcut.0.weight") != 0;
     if (has_sc) {
-        std::vector<float> ss, hs, wsv;
-        if (!b.w.bn(p + ".shortcut.1", true, ss, hs) || !b.w.pack_conv(p + ".shortcut.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
-        int F3, T3;
-        const int K2 = add_conv_taps(cs, x, 1, 1, 1, 1, 0, 0, sf, st_, K, &F3, &T3);
-        if (K2 < 0 || F3 != Fo || T3 != To) { set_err("internal: shortcut shape mismatch"); b.ok = false; return none; }
-        std::vector<float> wm((size_t)cout * (K + K2));
-        for (int r = 0; r < cout; ++r) {
-            memcpy(&wm[(size_t)r * (K + K2)], &w2[(size_t)r * K], (size_t)K * 4);
-            memcpy(&wm[(size_t)r * (K + K2) + K], &wsv[(size_t)r * K2], (size_t)K2 * 4);
-        }
-        w2.swap(wm);
-        K += K2;
-        for (int i = 0; i < cout; ++i) bias2[i] += hs[i];
+        if (!b.merge_shortcut(cs, p, x, sf, st_, o, w2, K, bias2)) return none;
     } else {
         cs.epi.res = x.p;
         cs.epi.res_ld = x.ld;
@@ -720,60 +730,28 @@ View basic_block(Builder& b, const std::string& p, const View& x, int cout, int 
 View bottleneck_block(Builder& b, const std::string& p, const View& x, int planes, int s, View h1buf, View h2buf, View obuf,
                       int lvl_in = 0, int lvl = 0) {
     std::vector<float> s1, h1, s2, h2, s3, h3, w1, w2, w3;
-    int co, ci, nt;
     View none;
     if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.bn(p + ".bn3", true, s3, h3) ||
-        !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co, &ci, &nt) || !b.w.pack_conv(p + ".conv2.weight", &s2, w2, &co, &ci, &nt) ||
-        !b.w.pack_conv(p + ".conv3.weight", &s3, w3, &co, &ci, &nt))
+        !b.w.pack_conv(p + ".conv1.weight", &s1, w1) || !b.w.pack_conv(p + ".conv2.weight", &s2, w2) || !b.w.pack_conv(p + ".conv3.weight", &s3, w3))
         return none;
     const int cout = 4 * planes;
     const int Fo = (x.F + 2 - 3) / s + 1, To = (x.T + 2 - 3) / s + 1;
-    View a = h1buf; a.B = x.B; a.F = x.F; a.T = x.T; a.C = planes; a.ld = planes;
-    View c = h2buf; c.B = x.B; c.F = Fo; c.T = To; c.C = planes; c.ld = planes;
-    View o = obuf; o.B = x.B; o.F = Fo; o.T = To; o.C = cout; o.ld = cout;
+    const View a = h1buf.shaped(x.B, x.F, x.T, planes), c = h2buf.shaped(x.B, Fo, To, planes), o = obuf.shaped(x.B, Fo, To, cout);
     WsEpi e1{};
     e1.bias = b.w.f32("bnh:" + p + ".bn1", h1);
     e1.act1 = WS_ACT_RELU;
     b.conv_simple(x, a, b.w.act("w:" + p + ".conv1", w1), 1, 1, 1, 1, 0, 0, 1, 1, e1);
     b.zero_tail(a, lvl_in);   // (masked plans) the 3x3 conv reads `a` across time
     if (!b.good()) return none;
-    {   // 3x3: halo-resident kernel when stride 1 and planes <= 128, else the generic conv-GEMM
-        const float* b2 = b.w.f32("bnh:" + p + ".bn2", h2);
-        const void* W2 = b.w.act("w:" + p + ".conv2", w2);
-        bool done = false;
-        if ((s == 1 || b.e.opt("conv3x3_strided", 1) != 0) && b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0) {
-            Op op;
-            bool unsupported = false;
-            if (make_conv3x3_op(a, c, W2, b2, nullptr, true, &op, &unsupported, s, s, b.lens(lvl))) { b.push(std::move(op)); done = true; }
-            else if (!unsupported) { b.ok = false; return none; }
-        }
-        if (!done) {
-            WsEpi e2{};
-            e2.bias = b2;
-            e2.act1 = WS_ACT_RELU;
-            b.conv_simple(a, c, W2, 3, 3, 1, 1, 1, 1, s, s, e2);
-        }
-    }
-    if (!b.good()) return none;
+    // (conv3 is 1x1: its input needs no zero rows behind the utterance's end)
+    if (!b.conv3x3(a, c, b.w.act("w:" + p + ".conv2", w2), b.w.f32("bnh:" + p + ".bn2", h2), WS_ACT_RELU, s, s, lvl, false)) return none;
     ConvSpec cs;
     cs.dt = b.e.act_dt;
     int F3, T3;
     int K = add_conv_taps(cs, c, 1, 1, 1, 1, 0, 0, 1, 1, 0, &F3, &T3);
     std::vector<float> bias3 = h3;
     if (b.e.sd.count(p + ".shortcut.0.weight") != 0) {
-        std::vector<float> ss, hs, wsv;
-        if (!b.w.bn(p + ".shortcut.1", true, ss, hs) || !b.w.pack_conv(p + ".shortcut.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
-        int F4, T4;
-        const int K2 = add_conv_taps(cs, x, 1, 1, 1, 1, 0, 0, s, s, K, &F4, &T4);
-        if (K2 < 0 || F4 != Fo || T4 != To) { set_err("internal: shortcut shape mismatch"); b.ok = false; return none; }
-        std::vector<float> wm((size_t)cout * (K + K2));
-        for (int r = 0; r < cout; ++r) {
-            memcpy(&wm[(size_t)r * (K + K2)], &w3[(size_t)r * K], (size_t)K * 4);
-            memcpy(&wm[(size_t)r * (K + K2) + K], &wsv[(size_t)r * K2], (size_t)K2 * 4);
-        }
-        w3.swap(wm);
-        K += K2;
-        for (int i = 0; i < cout; ++i) bias3[i] += hs[i];
+        if (!b.merge_shortcut(cs, p, x, s, s, o, w3, K, bias3)) return none;
     } else {
         cs.epi.res = x.p;
         cs.epi.res_ld = x.ld;
@@ -794,7 +772,7 @@ View stem(Builder& b, const std::string& convkey, const std::string& bnkey, View
     if (!b.w.bn(bnkey, true, s, h) || !b.w.pack_conv(convkey, &s, w9, &co, &ci, &nt)) return none;
     if (ci != 1 || nt != 9) { set_err(convkey + ": expected (Cout,1,3,3)"); b.ok = false; return none; }
     const int B = b.p.B, T = b.p.T, Fd = b.e.feat_dim;
-    View o = outbuf; o.B = B; o.F = Fd; o.T = T; o.C = co; o.ld = co;
+    const View o = outbuf.shaped(B, Fd, T, co);
     const float* wd = b.w.f32("w:" + convkey + ".stem", w9);   // [Cout][9] (tap = df*3 + dt)
     const float* hd = b.w.f32("bnh:" + bnkey, h);
     const float* fin = b.p.feats_in;
@@ -802,26 +780,26 @@ View stem(Builder& b, const std::string& convkey, const std::string& bnkey, View
     void* op = o.p;
     float* olo = (float*)o.plo;
     const int* l0 = b.lens(0);
-    set_op_trace("{\"kind\":\"stem\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tp("feats", fin) + "," + Builder::tp("w9", wd) + "," + Builder::tp("shift", hd) + "," +
-                 Builder::tview("out", o) + "," + Builder::ti("Fdim", Fd) + "," + Builder::tp("lens", l0) + "}");
-    b.push([=](cudaStream_t st) { return ws_launch_stem(fin, wd, hd, op, olo, dt, B, T, Fd, co, st, l0); }, "stem");
+    b.push([=](cudaStream_t st) { return ws_launch_stem(fin, wd, hd, op, olo, dt, B, T, Fd, co, st, l0); }, "stem",
+           "{\"kind\":\"stem\"," + ti("es", ws_esize(dt)) + "," + tp("feats", fin) + "," + tp("w9", wd) + "," + tp("shift", hd) + "," +
+           tview("out", o) + "," + ti("Fdim", Fd) + "," + tp("lens", l0) + "}");
     return o;
 }
 
 // TSTP over the last feature map + the segment layer(s) (resnet.py:187-204; the same tail closes Res2Net / ERes2Net,
-// res2net.py:186-199, eres2net.py:379-391)
+// res2net.py:186-199, eres2net.py:379-391, Gemini DF-ResNet and XVEC)
+// two_layers: embed_b = seg_2(seg_bn_1(relu(seg_1(stats)))) (two_emb_layer), else embed_a = seg_1(stats)
 // lvl: stride level of `cur` in length-masked plans (three stride-2 layers in ResNet / Res2Net, one in Gemini DF-ResNet)
-bool resnet_tail(Builder& b, const View& cur, int E, int lvl = 3) {
-    ws_engine& e = b.e;
-    const int B = b.p.B;
+bool resnet_tail(Builder& b, const View& cur, bool two_layers, int lvl = 3) {
+    const int B = b.p.B, E = b.e.embed_dim;
     const int sd = cur.C * cur.F;  // stats_dim
     float* stats = b.f32((size_t)B * 2 * sd);
     b.tstats(cur, nullptr, nullptr, stats, 2 * sd, sd, lvl);  // TSTP, index c*F' + f (pooling_layers.py:78-85)
     const HostT* w1 = b.w.get("seg_1.weight");
     if (!w1) return false;
     if ((int)w1->shape[1] != 2 * sd || (int)w1->shape[0] != E) { set_err("seg_1.weight shape mismatch"); return false; }
-    if (e.opt("two_emb_layer", 0)) {
-        // embed_b = seg_2(seg_bn_1(relu(embed_a))) (resnet.py:196-200): BN (affine=False) folded into seg_2
+    if (two_layers) {
+        // seg_bn_1 (affine=False) folded into seg_2 (resnet.py:196-200)
         float* ea = b.f32((size_t)B * E);
         std::vector<float> s, h;
         const HostT* w2 = b.w.get("seg_2.weight");
@@ -848,14 +826,9 @@ bool resnet_tail(Builder& b, const View& cur, int E, int lvl = 3) {
 // resnet.py:110-204
 bool build_resnet(Builder& b) {
     ws_engine& e = b.e;
-    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim, m = 32;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, m = 32;
     // largest activation map: the layer-1 output (m channels, x4 with Bottleneck blocks) at full (F, T)
-    const size_t big = (size_t)B * Fd * T * m * (e.bottleneck ? 4 : 1);
-    View bufs[4];
-    for (int i = 0; i < (e.bottleneck ? 4 : 3); ++i) {
-        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
-        if (e.split) bufs[i].plo = b.raw(big * 4);
-    }
+    const std::vector<View> bufs = b.ring(e.bottleneck ? 4 : 3, (size_t)B * Fd * T * m * (e.bottleneck ? 4 : 1));
     if (!b.good()) return false;
     View cur = stem(b, "conv1.weight", "bn1", bufs[0]);
     int ci = 0;
@@ -877,7 +850,7 @@ bool build_resnet(Builder& b) {
         }
     }
     if (!b.good()) return false;
-    return resnet_tail(b, cur, E);
+    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0);
 }
 
 // ----------------------------------------------------------------------------------------------- Res2Net / ERes2Net
@@ -926,17 +899,16 @@ static std::vector<float> pad_cols(const std::vector<float>& m, int R, int G, in
 static bool aff(Builder& b, const std::string& p, const View& x, const View& y, int Cr, View hidbuf, View attbuf, const View& out) {
     const int Cp = x.C, inter = Cr / 4, ip = std::max(32, (inter + 31) / 32 * 32);
     std::vector<float> sa, ha, sb, hb, wa, wb;
-    int co, ci, nt;
     const HostT* ba = b.w.get(p + ".local_att.0.bias");
     const HostT* bb = b.w.get(p + ".local_att.3.bias");
     if (!ba || !bb || !b.w.bn(p + ".local_att.1", true, sa, ha) || !b.w.bn(p + ".local_att.4", true, sb, hb) ||
-        !b.w.pack_conv(p + ".local_att.0.weight", &sa, wa, &co, &ci, &nt) || !b.w.pack_conv(p + ".local_att.3.weight", &sb, wb, &co, &ci, &nt))
+        !b.w.pack_conv(p + ".local_att.0.weight", &sa, wa) || !b.w.pack_conv(p + ".local_att.3.weight", &sb, wb))
         return false;
     if ((int)wa.size() != inter * 2 * Cr || (int)wb.size() != Cr * inter || y.C != Cp || Cr > Cp) { set_err(p + ": AFF weight shape mismatch"); b.ok = false; return false; }
     // conv a: rows inter -> ip, columns [x: Cr -> Cp | y: Cr -> Cp]
     std::vector<float> wap = pad_rows(pad_cols(wa, inter, 2, 1, Cr, Cp), 1, inter, ip, 2 * Cp), bap(ip, 0.f);
     for (int i = 0; i < inter; ++i) bap[i] = sa[i] * ba->v[i] + ha[i];
-    View hid = hidbuf; hid.B = x.B; hid.F = x.F; hid.T = x.T; hid.C = ip; hid.ld = ip;
+    const View hid = hidbuf.shaped(x.B, x.F, x.T, ip);
     {
         ConvSpec cs;
         cs.dt = b.e.act_dt;
@@ -954,7 +926,7 @@ static bool aff(Builder& b, const std::string& p, const View& x, const View& y, 
     // conv b: rows Cr -> Cp, columns inter -> ip; tanh in the epilogue
     std::vector<float> wbp = pad_rows(pad_cols(wb, Cr, 1, 1, inter, ip), 1, Cr, Cp, ip), bbp(Cp, 0.f);
     for (int i = 0; i < Cr; ++i) bbp[i] = sb[i] * bb->v[i] + hb[i];
-    View att = attbuf; att.B = x.B; att.F = x.F; att.T = x.T; att.C = Cp; att.ld = Cp;
+    const View att = attbuf.shaped(x.B, x.F, x.T, Cp);
     WsEpi eb{};
     eb.bias = b.w.f32("b:" + p + ".att3", bbp);
     eb.act1 = WS_ACT_TANH;
@@ -963,41 +935,22 @@ static bool aff(Builder& b, const std::string& p, const View& x, const View& y, 
     const View xv = x, yv = y, av = att, ov = out;
     const int dt = b.e.act_dt;
     const long long npos = x.npos();
-    set_op_trace("{\"kind\":\"aff_combine\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", xv) + "," + Builder::tview("y", yv) + "," + Builder::tview("t", av) + "," +
-                 Builder::tview("out", ov) + "}");
     b.push([=](cudaStream_t s) {
         return ws_launch_aff_combine(xv.p, xv.ld, yv.p, yv.ld, av.p, av.ld, ov.p, (float*)ov.plo, ov.ld, dt, npos, Cp, s);
-    }, "aff_combine");
+    }, "aff_combine", "{\"kind\":\"aff_combine\"," + ti("es", ws_esize(dt)) + "," + tview("x", xv) + "," + tview("y", yv) + "," + tview("t", av) + "," +
+                      tview("out", ov) + "}");
     return b.good();
 }
 
-// 3x3 pad-1 conv (+ folded BN shift) -> act over `in` (and, when in2 != nullptr, over in + in2 with the weights repeated):
-// the halo-resident kernel where it applies, else the generic conv-GEMM.  act: WS_ACT_RELU20, WS_ACT_RELU or WS_ACT_NONE.
-// stride_t: the time stride when it differs from the frequency stride `stride` (0: the same)
+// 3x3 pad-1 conv (+ folded BN shift) -> act over `in` (Builder::conv3x3), or, when in2 != nullptr, over in + in2 with the
+// weights repeated (the conv-GEMM).  act: WS_ACT_RELU20, WS_ACT_RELU or WS_ACT_NONE.  stride_t: the time stride when it
+// differs from the frequency stride `stride` (0: the same)
 static bool res2_conv3x3(Builder& b, const std::string& id, const View& in, const View* in2, const View& out, const std::vector<float>& w9,
                          const std::vector<float>& bias, int act, int stride, int lvl, int stride_t = 0) {   // lvl: stride level of `out` (length-masked plans)
     const int Cin = in.C, Cout = out.C, sf = stride, st = stride_t > 0 ? stride_t : stride;
     if ((int)w9.size() != Cout * 9 * Cin || (int)bias.size() != Cout) { set_err(id + ": 3x3 weight shape mismatch"); b.ok = false; return false; }
     const float* bd = b.w.f32("b:" + id, bias);
-    if (in2 == nullptr) {
-        const void* W = b.w.act("w:" + id, w9);
-        if (b.e.use_tc >= 2 && b.e.act_dt != WS_F32 && b.e.opt("conv3x3", 1) != 0 && ((sf == 1 && st == 1) || b.e.opt("conv3x3_strided", 1) != 0)) {
-            Op op;
-            bool unsupported = false;
-            if (make_conv3x3_op(in, out, W, bd, nullptr, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, &op, &unsupported, sf, st,
-                                b.lens(lvl))) {
-                b.push(std::move(op));
-                return b.good();
-            }
-            if (!unsupported) { b.ok = false; return false; }
-        }
-        WsEpi ep{};
-        ep.bias = bd;
-        ep.act1 = act;
-        b.conv_simple(in, out, W, 3, 3, 1, 1, 1, 1, sf, st, ep);
-        b.zero_tail(out, lvl);
-        return b.good();
-    }
+    if (in2 == nullptr) return b.conv3x3(in, out, b.w.act("w:" + id, w9), bd, act, sf, st, lvl);
     // two summed inputs: K = [9 taps over in | 9 taps over in2], weight rows repeated
     std::vector<float> w2((size_t)Cout * 18 * Cin);
     for (int o = 0; o < Cout; ++o) {
@@ -1035,14 +988,11 @@ static View res2_block(Builder& b, const Res2Cfg& c, const std::string& p, const
     const int ncat = kind == 0 ? s - 1 : s;             // chunks of the concat buffer (Res2Net's last chunk stays in A)
     const int Fo = (x.F - 1) / stride + 1, To = (x.T - 1) / stride + 1;
     std::vector<float> s1, h1, s3, h3, w1, w3;
-    int co, ci, nt;
-    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn3", true, s3, h3) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co, &ci, &nt) ||
-        !b.w.pack_conv(p + ".conv3.weight", &s3, w3, &co, &ci, &nt))
+    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn3", true, s3, h3) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1) ||
+        !b.w.pack_conv(p + ".conv3.weight", &s3, w3))
         return none;
     if ((int)w1.size() != s * w * cin || (int)w3.size() != cout * s * w) { set_err(p + ": conv1 / conv3 weight shape mismatch"); b.ok = false; return none; }
-    View A = bf.A; A.B = x.B; A.F = Fo; A.T = To; A.C = s * wp; A.ld = s * wp;
-    View cat = bf.cat; cat.B = x.B; cat.F = Fo; cat.T = To; cat.C = ncat * wp; cat.ld = ncat * wp;
-    View o = obuf; o.B = x.B; o.F = Fo; o.T = To; o.C = cout; o.ld = cout;
+    const View A = bf.A.shaped(x.B, Fo, To, s * wp), cat = bf.cat.shaped(x.B, Fo, To, ncat * wp), o = obuf.shaped(x.B, Fo, To, cout);
     {   // conv1 (1x1, stride) + bn1 + Hardtanh -> the `scale` chunks of A
         std::vector<float> w1p = pad_rows(w1, s, w, wp, cin), b1p((size_t)s * wp, 0.f);
         for (int k = 0; k < s; ++k)
@@ -1060,6 +1010,7 @@ static View res2_block(Builder& b, const Res2Cfg& c, const std::string& p, const
         const std::string bk = (kind == 2) ? (i == 0 ? p + ".bn2_1" : p + ".bns." + std::to_string(i - 1))
                                            : p + ".bns." + std::to_string(i);
         std::vector<float> sc, sh, wc;
+        int co, ci, nt;
         if (!b.w.bn(bk, true, sc, sh) || !b.w.pack_conv(ck + ".weight", &sc, wc, &co, &ci, &nt)) return none;
         if (co != w || ci != w || nt != 9) { set_err(ck + ".weight: expected (w, w, 3, 3)"); b.ok = false; return none; }
         // [w][9][w] -> [wp][9][wp]
@@ -1069,7 +1020,7 @@ static View res2_block(Builder& b, const Res2Cfg& c, const std::string& p, const
         if (i == 0) {
             if (!res2_conv3x3(b, ck, spx, nullptr, dst, wcp, bcp, WS_ACT_RELU20, 1, lvl)) return none;
         } else if (kind == 2) {
-            View fz = bf.fz; fz.B = x.B; fz.F = Fo; fz.T = To; fz.C = wp; fz.ld = wp;
+            const View fz = bf.fz.shaped(x.B, Fo, To, wp);
             if (!aff(b, p + ".fuse_models." + std::to_string(i - 1), cat.ch((i - 1) * wp, wp), spx, w, bf.hid, bf.att, fz)) return none;
             if (!res2_conv3x3(b, ck, fz, nullptr, dst, wcp, bcp, WS_ACT_RELU20, 1, lvl)) return none;
         } else {
@@ -1091,19 +1042,7 @@ static View res2_block(Builder& b, const Res2Cfg& c, const std::string& p, const
     std::vector<float> w3p = pad_cols(w3, cout, 1, s, w, wp), bias3 = h3;
     const bool has_sc = b.e.sd.count(p + ".shortcut.0.weight") != 0;
     if (has_sc) {
-        std::vector<float> ss, hs, wsv;
-        if (!b.w.bn(p + ".shortcut.1", true, ss, hs) || !b.w.pack_conv(p + ".shortcut.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
-        int F4, T4;
-        const int K2 = add_conv_taps(cs, x, 1, 1, 1, 1, 0, 0, stride, stride, K, &F4, &T4);
-        if (K2 != cin || co != cout || F4 != Fo || T4 != To) { set_err(p + ": shortcut shape mismatch"); b.ok = false; return none; }
-        std::vector<float> wm((size_t)cout * (K + K2));
-        for (int r = 0; r < cout; ++r) {
-            memcpy(&wm[(size_t)r * (K + K2)], &w3p[(size_t)r * K], (size_t)K * 4);
-            memcpy(&wm[(size_t)r * (K + K2) + K], &wsv[(size_t)r * K2], (size_t)K2 * 4);
-        }
-        w3p.swap(wm);
-        K += K2;
-        for (int i = 0; i < cout; ++i) bias3[i] += hs[i];
+        if (!b.merge_shortcut(cs, p, x, stride, stride, o, w3p, K, bias3)) return none;
     } else {
         if (cin != cout || stride != 1) { set_err(p + ": identity shortcut with a shape change"); b.ok = false; return none; }
         cs.epi.res = x.p;
@@ -1121,7 +1060,7 @@ static View res2_block(Builder& b, const Res2Cfg& c, const std::string& p, const
 
 bool build_res2net(Builder& b, const Res2Cfg& c) {
     ws_engine& e = b.e;
-    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim, m = c.m;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, m = c.m;
     if (m != 32 && m != 64) { set_err("Res2Net / ERes2Net: m_channels must be 32 or 64"); return false; }
     View stem_buf = b.act(B, Fd, T, m);
     if (!b.good()) return false;
@@ -1181,7 +1120,7 @@ bool build_res2net(Builder& b, const Res2Cfg& c) {
         cur = f;
     }
     if (!b.good()) return false;
-    return resnet_tail(b, cur, E);
+    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0);
 }
 
 // ----------------------------------------------------------------------------------------------- SimAM-ResNet + ASP
@@ -1200,16 +1139,14 @@ static bool simam(Builder& b, const View& y, const View& res, const View& out, W
     const WsMapStrides rs{(long long)res.F * res.T * res.ld, (long long)res.T * res.ld, res.ld};
     const int* l = b.lens(lvl);
     const int dt = b.e.act_dt;
-    set_op_trace("{\"kind\":\"simam_stats\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", yv) + "," + Builder::tp("stats", stats) + "," +
-                 Builder::tp("lens", l) + "}");
-    b.push([=](cudaStream_t s) { return ws_launch_simam_stats(yv.p, dt, yv.B, yv.F, yv.T, yv.C, yv.ld, partial, stats, s, l); }, "simam_stats");
+    b.push([=](cudaStream_t s) { return ws_launch_simam_stats(yv.p, dt, yv.B, yv.F, yv.T, yv.C, yv.ld, partial, stats, s, l); }, "simam_stats",
+           "{\"kind\":\"simam_stats\"," + ti("es", ws_esize(dt)) + "," + tview("x", yv) + "," + tp("stats", stats) + "," + tp("lens", l) + "}");
     b.p.extra_launches += 1;   // partials + merge
-    set_op_trace("{\"kind\":\"simam_apply\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("y", yv) + "," + Builder::tp("stats", stats) + "," +
-                 Builder::tview("res", rv) + "," + Builder::tp("out", op_) + "," + Builder::ti("out_sb", os.b) + "," + Builder::ti("out_sf", os.f) + "," +
-                 Builder::ti("out_st", os.t) + "," + Builder::tp("lens", l) + ",\"lambda\":1e-4}");
     b.push([=](cudaStream_t s) {
         return ws_launch_simam_apply(yv.p, yv.ld, stats, kSimamLambda, rv.p, rs, op_, olo, os, dt, yv.B, yv.F, yv.T, yv.C, s, l);
-    }, "simam_apply");
+    }, "simam_apply", "{\"kind\":\"simam_apply\"," + ti("es", ws_esize(dt)) + "," + tview("y", yv) + "," + tp("stats", stats) + "," +
+                      tview("res", rv) + "," + tp("out", op_) + "," + ti("out_sb", os.b) + "," + ti("out_sf", os.f) + "," +
+                      ti("out_st", os.t) + "," + tp("lens", l) + ",\"lambda\":1e-4}");
     return b.good();
 }
 
@@ -1219,19 +1156,17 @@ static View simam_block(Builder& b, const std::string& p, const View& x, int cou
                         float* partial, float* stats, const View* frame) {
     View none;
     std::vector<float> s1, h1, s2, h2, w1, w2;
-    int co, ci, nt;
-    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1, &co, &ci, &nt) ||
-        !b.w.pack_conv(p + ".conv2.weight", &s2, w2, &co, &ci, &nt))
+    if (!b.w.bn(p + ".bn1", true, s1, h1) || !b.w.bn(p + ".bn2", true, s2, h2) || !b.w.pack_conv(p + ".conv1.weight", &s1, w1) ||
+        !b.w.pack_conv(p + ".conv2.weight", &s2, w2))
         return none;
     const int Fo = (x.F - 1) / s + 1, To = (x.T - 1) / s + 1;
-    View h = hbuf; h.B = x.B; h.F = Fo; h.T = To; h.C = cout; h.ld = cout;
-    View y = ybuf; y.B = x.B; y.F = Fo; y.T = To; y.C = cout; y.ld = cout;
-    View o = obuf; o.B = x.B; o.F = Fo; o.T = To; o.C = cout; o.ld = cout;
+    const View h = hbuf.shaped(x.B, Fo, To, cout), y = ybuf.shaped(x.B, Fo, To, cout), o = obuf.shaped(x.B, Fo, To, cout);
     if (!res2_conv3x3(b, p + ".conv1", x, nullptr, h, w1, h1, WS_ACT_RELU, s, lvl) || !res2_conv3x3(b, p + ".conv2", h, nullptr, y, w2, h2, WS_ACT_NONE, 1, lvl))
         return none;
     const bool has_ds = b.e.sd.count(p + ".downsample.0.weight") != 0;
     if (has_ds) {
         std::vector<float> ss, hs, wsv;
+        int co, ci, nt;
         if (!b.w.bn(p + ".downsample.1", true, ss, hs) || !b.w.pack_conv(p + ".downsample.0.weight", &ss, wsv, &co, &ci, &nt)) return none;
         if (co != cout || ci != x.C || nt != 1) { set_err(p + ".downsample.0.weight: shape mismatch"); b.ok = false; return none; }
         WsEpi es{};
@@ -1260,12 +1195,7 @@ bool build_simam_resnet(Builder& b) {
     const int m = (int)c1->shape[0];   // in_planes
     if (m != 32 && m != 64) { set_err("SimAM-ResNet: in_planes (the rows of front.conv1.weight) must be 32 or 64"); return false; }
     // every map has F * C = feat_dim * in_planes (the stride-2 layers halve F and double C): a layer-1 tensor is the largest
-    const size_t big = (size_t)B * Fd * T * m;
-    View bufs[4];
-    for (int i = 0; i < 4; ++i) {
-        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
-        if (e.split) bufs[i].plo = b.raw(big * 4);
-    }
+    const std::vector<View> bufs = b.ring(4, (size_t)B * Fd * T * m);
     int F4 = Fd, T4 = T;
     for (int i = 0; i < 3; ++i) { F4 = (F4 - 1) / 2 + 1; T4 = (T4 - 1) / 2 + 1; }
     const int C4 = 8 * m, D = F4 * C4;   // ASP feature_dim = in_planes * 8 * (acoustic_dim / 8) (pooling_layers.py:167-170)
@@ -1320,26 +1250,7 @@ bool build_simam_resnet(Builder& b) {
     ep.scale = b.w.f32("bns:pooling.attention.2", sa);
     ep.shift = b.w.f32("bnh:pooling.attention.2", ha);
     b.conv_simple(frame, hid, b.w.act("w:pooling.attention.0", w0), 1, 1, 1, 1, 0, 0, 1, 1, ep);
-    const void* W3 = b.w.act("w:pooling.attention.3", w3);
-    const int* l3 = b.lens(3);
-    bool fused = false;
-    if (e.use_tc >= 2 && e.opt("astp_fused", 1) && b.good()) {   // attention.3's bias cancels in the softmax
-        Op op;
-        bool unsupported = false;
-        if (make_astp_op(frame, hid, W3, stats, 1e-5f, &op, &unsupported, l3)) { b.push(std::move(op)); fused = true; }
-        else if (!unsupported) return false;
-    }
-    if (!fused) {
-        View logits = b.act(B, 1, T4, D);
-        WsEpi ep3{};
-        ep3.bias = b.w.f32("b:pooling.attention.3", b3);
-        b.conv_simple(hid, logits, W3, 1, 1, 1, 1, 0, 0, 1, 1, ep3);
-        if (!b.good()) return false;
-        const View fr = frame, lg = logits;
-        set_op_trace("{\"kind\":\"astp_stats\"," + Builder::ti("es", ws_esize(fr.dt)) + "," + Builder::tview("x", fr) + "," + Builder::tview("logits", lg) + "," +
-                     Builder::tp("stats", stats) + "," + Builder::tp("lens", l3) + ",\"eps\":1e-05}");
-        b.push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, B, T4, D, fr.ld, stats, 1e-5f, s, l3); }, "astp_stats");
-    }
+    if (!b.astp_tail(frame, hid, b.w.act("w:pooling.attention.3", w3), b.w.f32("b:pooling.attention.3", b3), stats, 1e-5, 3)) return false;
     b.linear(stats, 2 * D, nullptr, 0, 1, b.w.f32("w:bottleneck.pooled", wb), b.w.vec("bottleneck.bias"), b.p.emb, E, B, 2 * D, E, WS_ACT_NONE);
     return b.good();
 }
@@ -1363,11 +1274,10 @@ static bool dwconv3x3(Builder& b, const std::string& id, const View& x, const Vi
     }
     const View xv = x, ov = out;
     const int* l = b.lens(lvl);
-    set_op_trace("{\"kind\":\"dwconv3x3\"," + Builder::ti("es", ws_esize(xv.dt)) + "," + Builder::tview("x", xv) + "," + Builder::tview("out", ov) + "," +
-                 Builder::tp("w", w9) + "," + Builder::tp("shift", shift) + "," + Builder::tp("lens", l) + "}");
     b.push([=](cudaStream_t s) {
         return ws_launch_dwconv3x3(xv.p, xv.ld, w9, shift, ov.p, (float*)ov.plo, ov.ld, xv.dt, xv.B, xv.F, xv.T, xv.C, s, l);
-    }, "dwconv3x3");
+    }, "dwconv3x3", "{\"kind\":\"dwconv3x3\"," + ti("es", ws_esize(xv.dt)) + "," + tview("x", xv) + "," + tview("out", ov) + "," +
+                    tp("w", w9) + "," + tp("shift", shift) + "," + tp("lens", l) + "}");
     return b.good();
 }
 
@@ -1391,9 +1301,7 @@ static View gemini_block(Builder& b, const std::string& p, const View& x, View h
     std::vector<float> w2((size_t)C4 * 9);   // [C4][3][3] with bn2's scale folded in
     for (int c = 0; c < C4; ++c)
         for (int k = 0; k < 9; ++k) w2[(size_t)c * 9 + k] = c2->v[(size_t)c * 9 + k] * s2[c];
-    View h = hbuf; h.B = x.B; h.F = x.F; h.T = x.T; h.C = C4; h.ld = C4;
-    View d = dbuf; d.B = x.B; d.F = x.F; d.T = x.T; d.C = C4; d.ld = C4;
-    View o = obuf; o.B = x.B; o.F = x.F; o.T = x.T; o.C = x.C; o.ld = x.C;
+    const View h = hbuf.shaped(x.B, x.F, x.T, C4), d = dbuf.shaped(x.B, x.F, x.T, C4), o = obuf.shaped(x.B, x.F, x.T, x.C);
     WsEpi e1{};
     e1.bias = b.w.f32("bnh:" + p + ".bn1", h1);
     e1.act1 = WS_ACT_RELU;
@@ -1411,7 +1319,7 @@ static View gemini_block(Builder& b, const std::string& p, const View& x, View h
 
 bool build_gemini(Builder& b) {
     ws_engine& e = b.e;
-    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim;
     int dims[5], Fs[5], Ts[5];
     Fs[0] = Fd; Ts[0] = T;
     for (int i = 0; i < 5; ++i) {
@@ -1435,12 +1343,7 @@ bool build_gemini(Builder& b) {
     // the largest map: the stem output or a stage's 4x-expanded tensor
     size_t big = (size_t)Fd * T * dims[0];
     for (int i = 1; i <= 4; ++i) big = std::max(big, (size_t)Fs[i] * Ts[i] * 4 * dims[i]);
-    big *= B;
-    View bufs[4];
-    for (int i = 0; i < 4; ++i) {
-        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
-        if (e.split) bufs[i].plo = b.raw(big * 4);
-    }
+    const std::vector<View> bufs = b.ring(4, big * B);
     if (!b.good()) return false;
     View cur = stem(b, "downsample_layers.0.0.weight", "downsample_layers.0.1", bufs[0]);
     if (!b.good() || cur.p == nullptr) return false;
@@ -1448,12 +1351,11 @@ bool build_gemini(Builder& b) {
     for (int i = 1; i <= 4; ++i) {
         const std::string p = "downsample_layers." + std::to_string(i);
         std::vector<float> s, h, w;
-        int co, cin, nt;
-        if (!b.w.bn(p + ".1", true, s, h) || !b.w.pack_conv(p + ".0.weight", &s, w, &co, &cin, &nt)) return false;
+        if (!b.w.bn(p + ".1", true, s, h) || !b.w.pack_conv(p + ".0.weight", &s, w)) return false;
         // stride levels of length-masked plans: 0 up to downsample_layers.2 (the only time stride), 1 behind it
         const int lvl_in = i >= 3 ? 1 : 0, lvl = i >= 2 ? 1 : 0;
         if (i >= 2) b.zero_tail(cur, lvl_in);   // (masked plans) a stage output, read across time by the 3x3 conv
-        View o = bufs[(ci + 1) % 4]; o.B = B; o.F = Fs[i]; o.T = Ts[i]; o.C = co; o.ld = co;
+        const View o = bufs[(ci + 1) % 4].shaped(B, Fs[i], Ts[i], dims[i]);
         if (!res2_conv3x3(b, p + ".0", cur, nullptr, o, w, h, WS_ACT_NONE, 2, lvl, kGeminiStrideT[i - 1])) return false;
         ci = (ci + 1) % 4;
         cur = o;
@@ -1465,7 +1367,7 @@ bool build_gemini(Builder& b) {
             cur = nx;
         }
     }
-    return resnet_tail(b, cur, E, 1);
+    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0, 1);
 }
 
 // ----------------------------------------------------------------------------------------------- XVEC
@@ -1473,24 +1375,15 @@ bool build_gemini(Builder& b) {
 // BatchNorm affine=False, TSTP, seg_1 -> ReLU -> seg_bn_1 -> seg_2; callers take the last element (embed_b).
 bool build_xvec(Builder& b) {
     ws_engine& e = b.e;
-    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim;
+    const int B = b.p.B, T = b.p.T, Fd = e.feat_dim;
     if (T < 15) { set_err("XVEC needs at least 15 frames (valid convolutions of context 5, 3x2, 3x3)"); return false; }
     if (b.p.masked) { set_err("length-masked batches are not implemented for XVEC (its valid convolutions shrink every utterance differently)"); return false; }
     const HostT* w5 = b.w.get("frame_5.conv_1d.weight");
-    const HostT* w1h = b.w.get("frame_1.conv_1d.weight");
-    if (!w5 || !w1h) return false;
-    const int hid = (int)w1h->shape[0], sdim = (int)w5->shape[0];
+    if (!w5) return false;
+    const int sdim = (int)w5->shape[0];
     const int sdim_pad = (sdim + 31) / 32 * 32;          // tensor-core tiles want Cout % 32 == 0: zero rows behind the 1500
     View x0 = b.act(B, 1, T, Fd);
-    {
-        const float* fin = b.p.feats_in;
-        void* xo = x0.p;
-        float* xlo = (float*)x0.plo;
-        const int dt = e.act_dt;
-        const long long n = (long long)B * T * Fd;
-        set_op_trace("{\"kind\":\"convert\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tp("in", fin) + "," + Builder::tp("out", xo) + "," + Builder::ti("n", n) + "}");
-        b.push([=](cudaStream_t s) { return ws_launch_convert(fin, xo, xlo, dt, n, s); }, "convert");
-    }
+    b.convert_input(x0);
     const int ks[5] = {5, 3, 3, 1, 1}, dils[5] = {1, 2, 3, 1, 1};
     View cur = x0;
     for (int i = 1; i <= 5 && b.good(); ++i) {
@@ -1514,31 +1407,10 @@ bool build_xvec(Builder& b) {
         ep.shift = b.w.f32("bnh:" + p, h);
         b.conv_simple(cur, out, b.w.act("w:" + p, wp), 1, ks[i - 1], 1, dils[i - 1], 0, 0, 1, 1, ep);
         cur = out;
-        (void)hid;
     }
     if (!b.good()) return false;
-    float* stats = b.f32((size_t)B * 2 * sdim);
     View sv = cur; sv.C = sdim;                           // statistics over the real 1500 channels only
-    b.tstats(sv, nullptr, nullptr, stats, 2 * sdim, sdim);
-    float* ea = b.f32((size_t)B * E);
-    std::vector<float> s, h;
-    const HostT* w1 = b.w.get("seg_1.weight");
-    const HostT* w2 = b.w.get("seg_2.weight");
-    const HostT* b2 = b.w.get("seg_2.bias");
-    if (!w1 || !w2 || !b2 || !b.w.bn("seg_bn_1", false, s, h)) return false;
-    if ((int)w1->shape[1] != 2 * sdim || (int)w1->shape[0] != E) { set_err("seg_1.weight shape mismatch"); return false; }
-    std::vector<float> wf((size_t)E * E), bf(E);
-    for (int o = 0; o < E; ++o) {
-        double acc = b2->v[o];
-        for (int i = 0; i < E; ++i) {
-            wf[(size_t)o * E + i] = w2->v[(size_t)o * E + i] * s[i];
-            acc += (double)w2->v[(size_t)o * E + i] * h[i];
-        }
-        bf[o] = (float)acc;
-    }
-    b.linear(stats, 2 * sdim, nullptr, 0, 1, b.w.vec("seg_1.weight"), b.w.vec("seg_1.bias"), ea, E, B, 2 * sdim, E, WS_ACT_RELU);
-    b.linear(ea, E, nullptr, 0, 1, b.w.f32("w:seg_2.folded", wf), b.w.f32("b:seg_2.folded", bf), b.p.emb, E, B, E, E, WS_ACT_NONE);
-    return b.good();
+    return resnet_tail(b, sv, true, 0);
 }
 
 // ----------------------------------------------------------------------------------------------- CAM++
@@ -1546,12 +1418,7 @@ bool build_xvec(Builder& b) {
 bool build_campplus(Builder& b) {
     ws_engine& e = b.e;
     const int B = b.p.B, T = b.p.T, Fd = e.feat_dim, E = e.embed_dim, m = 32;
-    const size_t big = (size_t)B * Fd * T * m;
-    View bufs[3];
-    for (int i = 0; i < 3; ++i) {
-        bufs[i].dt = e.act_dt; bufs[i].p = b.raw(big * ws_esize(e.act_dt));
-        if (e.split) bufs[i].plo = b.raw(big * 4);
-    }
+    const std::vector<View> bufs = b.ring(3, (size_t)B * Fd * T * m);
     if (!b.good()) return false;
     // FCM head (campplus.py:282-330): frequency-only striding
     View cur = stem(b, "head.conv1.weight", "head.bn1", bufs[0]);
@@ -1564,31 +1431,12 @@ bool build_campplus(Builder& b) {
             cur = o;
         }
     if (!b.good()) return false;
-    View y;
+    const View y = bufs[(ci + 1) % 3].shaped(B, (cur.F + 2 - 3) / 2 + 1, cur.T, m);
     {
         std::vector<float> s, h, wp;
-        int co, cin, nt;
-        if (!b.w.bn("head.bn2", true, s, h) || !b.w.pack_conv("head.conv2.weight", &s, wp, &co, &cin, &nt)) return false;
-        y = bufs[(ci + 1) % 3];
-        y.B = B; y.F = (cur.F + 2 - 3) / 2 + 1; y.T = cur.T; y.C = m; y.ld = m;
-        const float* hb = b.w.f32("bnh:head.bn2", h);
-        const void* Wh = b.w.act("w:head.conv2", wp);
-        bool done = false;
-        if (e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("conv3x3", 1) != 0 && e.opt("conv3x3_strided", 1) != 0) {
-            Op op;
-            bool unsupported = false;
-            if (make_conv3x3_op(cur, y, Wh, hb, nullptr, true, &op, &unsupported, 2, 1, b.lens(0))) { b.push(std::move(op)); done = true; }
-            else if (!unsupported) return false;
-        }
-        if (!done) {
-            WsEpi ep{};
-            ep.bias = hb;
-            ep.act1 = WS_ACT_RELU;
-            b.conv_simple(cur, y, Wh, 3, 3, 1, 1, 1, 1, 2, 1, ep);
-            b.zero_tail(y, 0);
-        }
+        if (!b.w.bn("head.bn2", true, s, h) || !b.w.pack_conv("head.conv2.weight", &s, wp)) return false;
+        if (!b.conv3x3(cur, y, b.w.act("w:head.conv2", wp), b.w.f32("bnh:head.bn2", h), WS_ACT_RELU, 2, 1, 0)) return false;
     }
-    if (!b.good()) return false;
     // xvector.tdnn: Conv1d(C*F -> 128, k5, stride 2, pad 2) on the (B, C*F, T) reshape (channel = c*F + f),
     // + BN + ReLU (campplus.py:345-355).  The frequency index becomes a tap dimension (df = f), stride 2 uses
     // the two time-parity planes.
@@ -1645,7 +1493,6 @@ bool build_campplus(Builder& b) {
         b.conv(cs);
     }
     const int dt = e.act_dt;
-    const long long npos = (long long)B * Tp;
     // Fused dense layers (ws_cam_dense.cu): one launch per CAMDenseTDNNLayer (or per block with cam_block = 1) instead of four
     const bool cam_fused = e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("cam_fused", 1) != 0 && Tp <= 512;
     for (int bl = 0; bl < 3 && b.good(); ++bl) {
@@ -1658,12 +1505,10 @@ bool build_campplus(Builder& b) {
                 const std::string p = "xvector.block" + std::to_string(bl + 1) + ".tdnnd" + std::to_string(j);
                 const int cin = c0[bl] + (j - 1) * growth;
                 std::vector<float> s1, h1, s2, h2, w1, wl;
-                int co, ci2, nt;
                 const HostT* c1w = b.w.get(p + ".cam_layer.linear1.weight");
                 const HostT* c2w = b.w.get(p + ".cam_layer.linear2.weight");
                 okl = c1w && c2w && b.w.bn(p + ".nonlinear1.batchnorm", true, s1, h1) && b.w.bn(p + ".nonlinear2.batchnorm", true, s2, h2) &&
-                      b.w.pack_conv(p + ".linear1.weight", &s2, w1, &co, &ci2, &nt) &&
-                      b.w.pack_conv(p + ".cam_layer.linear_local.weight", nullptr, wl, &co, &ci2, &nt);
+                      b.w.pack_conv(p + ".linear1.weight", &s2, w1) && b.w.pack_conv(p + ".cam_layer.linear_local.weight", nullptr, wl);
                 if (!okl) break;
                 std::vector<float> w1ct((size_t)bnc * (bnc / 2)), w2ct((size_t)(bnc / 2) * growth);
                 for (int o = 0; o < bnc / 2; ++o)
@@ -1681,9 +1526,9 @@ bool build_campplus(Builder& b) {
                 const float* b2cd = b.w.vec(p + ".cam_layer.linear2.bias");
                 okl = cam_layer_fill(&hl[(size_t)j - 1], e.act_dt, W1d, Wld, s1d, h1d, h2d, w1cd, b1cd, w2cd, b2cd, cin, dil[bl]);
                 if (plan_check_mode())
-                    hl_trace[(size_t)j - 1] = "{" + Builder::tp("W1", W1d) + "," + Builder::tp("Wl", Wld) + "," + Builder::tp("bn1_scale", s1d) + "," + Builder::tp("bn1_shift", h1d) +
-                                              "," + Builder::tp("bias2", h2d) + "," + Builder::tp("w1c_t", w1cd) + "," + Builder::tp("b1c", b1cd) + "," + Builder::tp("w2c_t", w2cd) + "," +
-                                              Builder::tp("b2c", b2cd) + "," + Builder::ti("cin", cin) + "," + Builder::ti("dil", dil[bl]) + "}";
+                    hl_trace[(size_t)j - 1] = "{" + tp("W1", W1d) + "," + tp("Wl", Wld) + "," + tp("bn1_scale", s1d) + "," + tp("bn1_shift", h1d) +
+                                              "," + tp("bias2", h2d) + "," + tp("w1c_t", w1cd) + "," + tp("b1c", b1cd) + "," + tp("w2c_t", w2cd) + "," +
+                                              tp("b2c", b2cd) + "," + ti("cin", cin) + "," + ti("dil", dil[bl]) + "}";
             }
             if (!okl || !b.good()) { b.ok = false; break; }
             const WsCamLayer* ldev = (const WsCamLayer*)b.w.upload("camlayers:" + std::to_string(bl), hl.data(), hl.size() * sizeof(WsCamLayer));
@@ -1691,15 +1536,15 @@ bool build_campplus(Builder& b) {
             const bool whole = e.opt("cam_block", 1) != 0;
             fused_done = true;
             for (int j = 0; j < nl[bl]; j += whole ? nl[bl] : 1) {
-                Op op;
+                const int j1 = whole ? nl[bl] : j + 1;
+                PlanOp op;
                 bool unsupported = false;
-                if (make_cam_dense_op(X[bl], ldev, j, whole ? nl[bl] : j + 1, &op, &unsupported, b.lens(1))) {
+                if (make_cam_dense_op(X[bl], ldev, j, j1, &op, &unsupported, b.lens(1))) {
                     if (plan_check_mode()) {   // semantic description of the fused launch: layers [j, j1) over the concat buffer
-                        const int j1 = whole ? nl[bl] : j + 1;
-                        std::string tr = "{\"kind\":\"cam_dense\"," + Builder::ti("es", ws_esize(e.act_dt)) + "," + Builder::tview("X", X[bl]) + "," + Builder::tp("lens", b.lens(1)) +
-                                         "," + Builder::ti("seg_len", 100) + ",\"layers\":[";
-                        for (int k = j; k < j1; ++k) tr += std::string(k > j ? "," : "") + hl_trace[(size_t)k];
-                        set_op_trace(tr + "]}");
+                        op.trace = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(e.act_dt)) + "," + tview("X", X[bl]) + "," + tp("lens", b.lens(1)) + "," +
+                                   ti("seg_len", 100) + ",\"layers\":[";
+                        for (int k = j; k < j1; ++k) op.trace += std::string(k > j ? "," : "") + hl_trace[(size_t)k];
+                        op.trace += "]}";
                     }
                     b.push(std::move(op));
                 }
@@ -1713,19 +1558,12 @@ bool build_campplus(Builder& b) {
             const std::string p = "xvector.block" + std::to_string(bl + 1) + ".tdnnd" + std::to_string(j);
             const int cin = c0[bl] + (j - 1) * growth;
             std::vector<float> s1, h1, s2, h2, w1, wl;
-            int co, ci2, nt;
             if (!b.w.bn(p + ".nonlinear1.batchnorm", true, s1, h1) || !b.w.bn(p + ".nonlinear2.batchnorm", true, s2, h2) ||
-                !b.w.pack_conv(p + ".linear1.weight", &s2, w1, &co, &ci2, &nt) ||
-                !b.w.pack_conv(p + ".cam_layer.linear_local.weight", nullptr, wl, &co, &ci2, &nt))
+                !b.w.pack_conv(p + ".linear1.weight", &s2, w1) || !b.w.pack_conv(p + ".cam_layer.linear_local.weight", nullptr, wl))
                 break;
             // nonlinear1 (BN-ReLU on the growing concat) -> scratch
-            View xs = X[bl].ch(0, cin);
-            View sv = scratch; sv.C = cin; sv.ld = cin;
-            const float* s1d = b.w.f32("bns:" + p + ".n1", s1);
-            const float* h1d = b.w.f32("bnh:" + p + ".n1", h1);
-            set_op_trace("{\"kind\":\"bnrelu\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", xs) + "," + Builder::tp("scale", s1d) + "," + Builder::tp("shift", h1d) + "," +
-                         Builder::tview("out", sv) + "," + Builder::ti("C", cin) + "}");
-            b.push([=](cudaStream_t st) { return ws_launch_bnrelu(xs.p, xs.ld, s1d, h1d, sv.p, (float*)sv.plo, sv.ld, dt, npos, cin, st); }, "bnrelu");
+            const View sv = scratch.shaped(B, 1, Tp, cin);
+            b.bnrelu(X[bl].ch(0, cin), b.w.f32("bns:" + p + ".n1", s1), b.w.f32("bnh:" + p + ".n1", h1), sv);
             // linear1 (1x1, no bias) + nonlinear2 (BN folded) + ReLU -> hid
             WsEpi e1{};
             e1.bias = b.w.f32("bnh:" + p + ".n2", h2);
@@ -1740,16 +1578,15 @@ bool build_campplus(Builder& b) {
                 const float* b2c = b.w.vec(p + ".cam_layer.linear2.bias");
                 const size_t cam_smem = (size_t)((bnc / 2) * bnc + nseg * bnc + 16 * bnc + nseg * (bnc / 2) + bnc) * 4;
                 if (cam_smem <= 48 * 1024) {
-                    set_op_trace("{\"kind\":\"cam_gate\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", hv) + "," + Builder::ti("seg_len", 100) + "," + Builder::tp("W1", w1c) + "," +
-                                 Builder::tp("b1", b1c) + "," + Builder::tp("W2", w2c) + "," + Builder::tp("b2", b2c) + "," + Builder::ti("H", bnc / 2) + "," + Builder::ti("G", growth) + "," +
-                                 Builder::tp("gate", cgate) + "}");
                     b.push([=](cudaStream_t st) {
                         return ws_launch_cam_gate(hv.p, dt, B, Tp, bnc, hv.ld, 100, w1c, b1c, w2c, b2c, bnc / 2, growth, cgate, st);
-                    }, "cam_gate");
+                    }, "cam_gate", "{\"kind\":\"cam_gate\"," + ti("es", ws_esize(dt)) + "," + tview("x", hv) + "," + ti("seg_len", 100) + "," + tp("W1", w1c) + "," +
+                                   tp("b1", b1c) + "," + tp("W2", w2c) + "," + tp("b2", b2c) + "," + ti("H", bnc / 2) + "," + ti("G", growth) + "," +
+                                   tp("gate", cgate) + "}");
                 } else {  // very long utterances: unfused path
-                    set_op_trace("{\"kind\":\"seg_means\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", hv) + "," + Builder::ti("seg_len", 100) + "," + Builder::tp("mean", cmean) + "," +
-                                 Builder::tp("segmean", csegm) + "}");
-                    b.push([=](cudaStream_t st) { return ws_launch_seg_means(hv.p, dt, B, Tp, bnc, hv.ld, 100, cmean, csegm, st); }, "seg_means");
+                    b.push([=](cudaStream_t st) { return ws_launch_seg_means(hv.p, dt, B, Tp, bnc, hv.ld, 100, cmean, csegm, st); }, "seg_means",
+                           "{\"kind\":\"seg_means\"," + ti("es", ws_esize(dt)) + "," + tview("x", hv) + "," + ti("seg_len", 100) + "," + tp("mean", cmean) + "," +
+                           tp("segmean", csegm) + "}");
                     b.linear(csegm, bnc, cmean, bnc, nseg, w1c, b1c, chid, bnc / 2, B * nseg, bnc, bnc / 2, WS_ACT_RELU);
                     b.linear(chid, bnc / 2, nullptr, 0, 1, w2c, b2c, cgate, growth, B * nseg, bnc / 2, growth, WS_ACT_SIGMOID);
                 }
@@ -1761,21 +1598,14 @@ bool build_campplus(Builder& b) {
         }
         if (!b.good()) break;
         // TransitLayer (campplus.py:204-218): BN-ReLU-Conv1x1 (no bias)
-        const std::string tp = "xvector.transit" + std::to_string(bl + 1);
+        const std::string tk = "xvector.transit" + std::to_string(bl + 1);
         std::vector<float> s, h, wt;
-        int co, ci2, nt;
-        if (!b.w.bn(tp + ".nonlinear.batchnorm", true, s, h) || !b.w.pack_conv(tp + ".linear.weight", nullptr, wt, &co, &ci2, &nt)) break;
-        View xs = X[bl];
-        View sv = scratch; sv.C = cmax[bl]; sv.ld = cmax[bl];
-        const float* sd_ = b.w.f32("bns:" + tp, s);
-        const float* hd_ = b.w.f32("bnh:" + tp, h);
-        const int cc = cmax[bl];
-        set_op_trace("{\"kind\":\"bnrelu\"," + Builder::ti("es", ws_esize(dt)) + "," + Builder::tview("x", xs) + "," + Builder::tp("scale", sd_) + "," + Builder::tp("shift", hd_) + "," +
-                     Builder::tview("out", sv) + "," + Builder::ti("C", cc) + "}");
-        b.push([=](cudaStream_t st) { return ws_launch_bnrelu(xs.p, xs.ld, sd_, hd_, sv.p, (float*)sv.plo, sv.ld, dt, npos, cc, st); }, "bnrelu");
+        if (!b.w.bn(tk + ".nonlinear.batchnorm", true, s, h) || !b.w.pack_conv(tk + ".linear.weight", nullptr, wt)) break;
+        const View sv = scratch.shaped(B, 1, Tp, cmax[bl]);
+        b.bnrelu(X[bl], b.w.f32("bns:" + tk, s), b.w.f32("bnh:" + tk, h), sv);
         WsEpi et{};
         View dst = (bl < 2) ? X[bl + 1].ch(0, cmax[bl] / 2) : Xf;
-        b.conv_simple(sv, dst, b.w.act("w:" + tp, wt), 1, 1, 1, 1, 0, 0, 1, 1, et);
+        b.conv_simple(sv, dst, b.w.act("w:" + tk, wt), 1, 1, 1, 1, 0, 0, 1, 1, et);
     }
     if (!b.good()) return false;
     {   // out_nonlinear (BN-ReLU) fused into TSTP; dense (1024 -> E, no bias) + BN(affine=False) folded
@@ -1811,8 +1641,8 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
         p->lens = (int*)b.raw((size_t)4 * B * sizeof(int));
         int* l = p->lens;
         if (b.good()) {
-            set_op_trace("{\"kind\":\"lens_derive\"," + Builder::tp("lens", l) + "," + Builder::ti("B", B) + "," + Builder::ti("T", T) + "," + Builder::ti("levels", 4) + "}");
-            b.push([=](cudaStream_t s) { return ws_launch_lens_derive(l, B, T, 4, s); }, "lens_derive");
+            b.push([=](cudaStream_t s) { return ws_launch_lens_derive(l, B, T, 4, s); }, "lens_derive",
+                   "{\"kind\":\"lens_derive\"," + tp("lens", l) + "," + ti("B", B) + "," + ti("T", T) + "," + ti("levels", 4) + "}");
         }
     }
     p->feats_in = b.f32((size_t)B * T * e->feat_dim);
@@ -1859,7 +1689,7 @@ int run_plan(ws_engine* e, Plan* p, cudaStream_t s) {
         cudaGraph_t g = nullptr;
         if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
             const char* m = nullptr;
-            for (auto& op : p->ops) { m = op(s); if (m) break; }
+            for (auto& op : p->ops) { m = op.run(s); if (m) break; }
             cudaError_t ce = cudaStreamEndCapture(s, &g);
             if (m == nullptr && ce == cudaSuccess && g != nullptr &&
                 cudaGraphInstantiate(&p->gexec, g, 0) == cudaSuccess) {
@@ -1878,7 +1708,7 @@ int run_plan(ws_engine* e, Plan* p, cudaStream_t s) {
     if (p->gexec != nullptr) {
         WS_CK(cudaGraphLaunch(p->gexec, s));
     } else {
-        for (auto& op : p->ops) WS_CKS(op(s));
+        for (auto& op : p->ops) WS_CKS(op.run(s));
     }
     e->last_launches = (long long)p->ops.size() + p->extra_launches;
     return 0;
@@ -2409,7 +2239,7 @@ int ws_engine_profile_ops(ws_engine* e, int B, int T, int iters, float* ms_out, 
     for (int it = 0; it < iters + 1; ++it) {
         cudaEventRecord(ev[0], e->st);
         for (int i = 0; i < n; ++i) {
-            const char* m = p->ops[i](e->st);
+            const char* m = p->ops[i].run(e->st);
             if (m) { set_err(std::string("profile_ops launch: ") + m); return -1; }
             cudaEventRecord(ev[i + 1], e->st);
         }
@@ -2430,9 +2260,9 @@ int ws_engine_profile_ops(ws_engine* e, int B, int T, int iters, float* ms_out, 
 const char* ws_engine_plan_op_name(ws_engine* e, int B, int T, int i, double* flops_out) {
     if (!e || !e->finalized || (!e->plan_check && cudaSetDevice(e->device) != cudaSuccess)) return nullptr;
     Plan* p = get_plan(e, B, T);
-    if (!p || i < 0 || i >= (int)p->op_names.size()) return nullptr;
-    if (flops_out) *flops_out = p->op_flops[i];
-    return p->op_names[i].c_str();
+    if (!p || i < 0 || i >= (int)p->ops.size()) return nullptr;
+    if (flops_out) *flops_out = p->ops[i].flops;
+    return p->ops[i].label.c_str();
 }
 
 // Plan-check engines only: write the (B,T) launch plan as data - a JSON description of every op (operands as placeholder
@@ -2446,8 +2276,8 @@ int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* pat
     Plan* p = get_plan(e, B, T, masked != 0);
     if (!p) return 1;
     std::string j = "{";
-    j += Builder::ti("B", B) + "," + Builder::ti("T", T) + "," + Builder::ti("feat_dim", e->feat_dim) + "," + Builder::ti("embed_dim", e->embed_dim) + "," +
-         Builder::ti("act_es", ws_esize(e->act_dt)) + "," + Builder::tp("feats_in", p->feats_in) + "," + Builder::tp("emb", p->emb) + "," + Builder::tp("lens", p->lens) + ",\"model\":\"" + e->model +
+    j += ti("B", B) + "," + ti("T", T) + "," + ti("feat_dim", e->feat_dim) + "," + ti("embed_dim", e->embed_dim) + "," +
+         ti("act_es", ws_esize(e->act_dt)) + "," + tp("feats_in", p->feats_in) + "," + tp("emb", p->emb) + "," + tp("lens", p->lens) + ",\"model\":\"" + e->model +
          "\",\"precision\":\"" + e->prec + "\",\"allocs\":[";
     for (size_t i = 0; i < e->check_allocs.size(); ++i)
         j += std::string(i ? "," : "") + "[" + std::to_string(e->check_allocs[i].first) + "," + std::to_string(e->check_allocs[i].second) + "]";
@@ -2461,9 +2291,9 @@ int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* pat
     }
     j += "],\"ops\":[";
     for (size_t i = 0; i < p->ops.size(); ++i) {
-        std::string lab = p->op_names[i];
+        std::string lab = p->ops[i].label;
         for (char& ch : lab) if (ch == '"' || ch == '\\') ch = ' ';
-        j += std::string(i ? "," : "") + "{\"label\":\"" + lab + "\",\"trace\":" + (p->op_traces[i].empty() ? std::string("null") : p->op_traces[i]) + "}";
+        j += std::string(i ? "," : "") + "{\"label\":\"" + lab + "\",\"trace\":" + (p->ops[i].trace.empty() ? std::string("null") : p->ops[i].trace) + "}";
     }
     j += "]}";
     FILE* f = fopen(path, "wb");

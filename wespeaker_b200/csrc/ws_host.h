@@ -1,6 +1,7 @@
 // Host-side plumbing shared by the engine translation units: error reporting, activation views, the conv
 // operator builder (wgmma/TMA or FFMA), device allocation tracking.
 #pragma once
+#include <cstdio>
 #include <functional>
 #include <map>
 #include <string>
@@ -11,9 +12,6 @@
 namespace ws {
 
 void set_err(const std::string& msg);
-// tuning aid: op factories leave a label (+ FLOPs) for the op they just built; Builder::push() attaches it to the plan
-void set_op_label(const std::string& name, double flops = 0.0);
-bool take_op_label(std::string* name, double* flops);
 const std::string& get_err();
 
 #define WS_CK(call)                                                                               \
@@ -43,11 +41,6 @@ struct PlanCheckScope {
     ~PlanCheckScope();
 };
 void* plan_check_alloc(size_t bytes);   // 256-byte aligned placeholder address
-// Plan trace (plan-check mode only, ws_engine_plan_trace): op factories leave a JSON description of the op they just built
-// (operands as placeholder addresses, shapes, strides, epilogue) and Builder::push() attaches it to the plan, so that a test
-// can re-evaluate the plan's arithmetic on the host and compare it with the oracle.  Outside plan-check mode these are no-ops.
-void set_op_trace(const std::string& json);
-bool take_op_trace(std::string* json);
 
 // channels-last activation view: element (b,f,t,c) at p[((b*F+f)*T+t)*ld + c]
 struct View {
@@ -57,6 +50,12 @@ struct View {
     long long ld = 0;
     int dt = WS_F32;
     long long npos() const { return (long long)B * F * T; }
+    // the same buffer as a dense (B, F, T, C) tensor
+    View shaped(int b, int f, int t, int c) const {
+        View v = *this;
+        v.B = b; v.F = f; v.T = t; v.C = c; v.ld = c;
+        return v;
+    }
     View ch(int c0, int c) const {
         View v = *this;
         v.p = (char*)p + (size_t)c0 * ws_esize(dt);
@@ -88,9 +87,27 @@ int add_conv_taps(ConvSpec& spec, const View& x, int kf, int kt, int dil_f, int 
                   int stride_f, int stride_t, int wk0, int* Fo, int* To);
 
 using Op = std::function<const char*(cudaStream_t)>;
+// One op of a launch plan: the launch closure, a label and FLOPs (tuning aid, ws_engine_profile_ops; FLOPs 0 = not GEMM-like)
+// and, in plan-check mode only, a JSON description of the op (operands as placeholder addresses, shapes, strides, epilogue)
+// that ws_engine_plan_trace writes so that a test can re-evaluate the plan's arithmetic on the host against the oracle.
+struct PlanOp {
+    Op run;
+    std::string label;
+    double flops = 0;
+    std::string trace;
+};
+
+// Plan-trace JSON fields: "name":address, "name":integer, "name":float (%.9g), "name":{view}
+inline std::string tp(const char* n, const void* q) { char b[96]; snprintf(b, sizeof b, "\"%s\":%llu", n, (unsigned long long)q); return b; }
+inline std::string ti(const char* n, long long v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%lld", n, v); return b; }
+inline std::string tf(const char* n, double v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%.9g", n, v); return b; }
+inline std::string tview(const char* n, const View& v) {
+    return std::string("\"") + n + "\":{" + tp("p", v.p) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
+}
+
 // Build a launch closure for `spec`; use_tc selects a tensor-core kernel (needs dt-aligned shapes) else FFMA.
 // Returns false and sets the error string if the spec cannot be mapped.
-bool make_conv_op(const ConvSpec& spec, int use_tc, Op* out);  // 0 FFMA, 1 tensor-core v1, 2 persistent v2 (falls back to v1), 3 v2 with clusters on large layers
+bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out);  // 0 FFMA, 1 tensor-core v1, 2 persistent v2 (falls back to v1), 3 v2 with clusters on large layers
 
 void fill_epi_out(WsEpi& e, const View& out);
 
@@ -99,13 +116,13 @@ void fill_epi_out(WsEpi& e, const View& out);
 // the activation dtype; bias/scale/shift: [7][w8] fp32.  Returns false with *unsupported=true when the shape/dtype is
 // outside the fused kernel's envelope (16-bit activations, w8 in {64,128}, T <= 256).
 bool make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
-                  const float* shift, int w8, int dil, Op* op, bool* unsupported, const int* lens = nullptr);
+                  const float* shift, int w8, int dil, PlanOp* op, bool* unsupported, const int* lens = nullptr);
 
 // Fused ASTP tail (ws_astp_fused.cu): x = frame-level features (B,1,T,C), h = the attention's hidden layer (B,1,T,128), W2 =
 // linear2 weight [C][128] in the activation dtype, stats = fp32 [B][2C] (weighted mean, std = sqrt(max(var, var_floor))).
 // linear2's bias cancels in the softmax over time and is not needed.  *unsupported = true outside the envelope (fp32
 // activations, C % 128, hidden width != 128).
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, Op* op, bool* unsupported,
+bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, bool* unsupported,
                   const int* lens = nullptr);
 
 // Halo-resident 3x3 pad-1 conv (ws_conv3x3.cu), strides 1 or 2 per axis: out = act(conv(x, W) + bias [+ res]).  x/out/res:
@@ -113,7 +130,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
 // 1 ReLU, 2 Hardtanh(0, 20).  Returns false with
 // *unsupported = true when the shape is outside the kernel's envelope (the caller then uses make_conv_op).
 bool make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
-                     Op* op, bool* unsupported, int stride_f = 1, int stride_t = 1, const int* lens = nullptr);
+                     PlanOp* op, bool* unsupported, int stride_f = 1, int stride_t = 1, const int* lens = nullptr);
 
 // Fused CAM++ dense layers (ws_cam_dense.cu).  cam_layer_fill builds one host-side layer descriptor (weights are device
 // pointers in the activation dtype: W1 [128][cin] with BN2 folded, Wl [32][3*128] tap-major; everything else fp32 device
@@ -122,7 +139,7 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
 bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const float* bn1_scale, const float* bn1_shift,
                     const float* bias2, const float* w1c_t, const float* b1c, const float* w2c_t, const float* b2c, int cin,
                     int dil);
-bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, Op* op, bool* unsupported,
+bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, bool* unsupported,
                        const int* lens = nullptr);
 
 }  // namespace ws
