@@ -9,6 +9,7 @@
 
 #include "../../include/wespeaker_b200.h"
 #include "ws_host.h"
+#include "ws_tc_common.cuh"   // ws_tc_lean_kind: which epilogue a layer takes decides whether it may use 256-wide tiles
 
 namespace ws {
 
@@ -293,21 +294,36 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     q->nout = (s.split ? 2 : 1) * (q->has_out2 ? 2 : 1);
     const int nstage_bufs = q->nout + (q->has_epin ? 1 : 0);
     const int budget = ws_tc2_max_smem() - 1024;
-    // widest N tile whose staging + >=3 ring stages fit (>=2 accepted as a last resort); 128 is the widest tile whose
-    // 64-row register accumulator (64 fp32 per thread) leaves the epilogue room in the consumer warpgroups
+    { const char* eg = getenv("WS_EPI_GENERIC"); q->epi_generic = eg != nullptr && atoi(eg) != 0; }
+    const int mtiles = q->tiles_t * q->tiles_f * q->tiles_b;
+    const int g_num_sms = ws_num_sms();
+    int ncl = g_num_sms;                       // clusters (or CTAs) resident at once
+    if (pair) {
+        ncl = ws_tc3_max_clusters(cl);
+        if (ncl <= 0) ncl = g_num_sms / cl;
+    }
+    // rounds of the persistent schedule: tiles of bn columns over ncl clusters
+    auto rounds = [&](int c) { return ((long long)(s.Cout / c) * ((mtiles + cl - 1) / cl) + ncl - 1) / ncl; };
+    // 256-wide tiles (16-bit, lean epilogue, no epilogue-input tile, 128-byte k-blocks; one 128-column staging buffer)
+    // halve the A-operand reads and the epilogue passes per FLOP, but a tile is twice the work: taken when the schedule
+    // then needs at most 10 % more time than with 128-wide tiles, counted in 128-wide rounds (20 r256 <= 11 r128)
+    q->epi = e; q->bn = 256; q->panel_bytes = 128;
+    const bool wide_ok = s.Cout % 256 == 0 && q->kind == 1 && !q->has_epin && q->bk_bytes == 128 && !q->epi_generic &&
+                         ws_tc_lean_kind(q) == s.dt + 1 && 20 * rounds(256) <= 11 * rounds(128);
+    // widest N tile whose staging + >=3 ring stages fit (>=2 accepted as a last resort, never for 256)
     int bn = 0, nst = 0;
     const int cands[4] = {256, 128, 64, 32};
     const char* env_bn = getenv("WS_TC2_MAX_BN");
-    const int max_bn = std::min(128, env_bn ? atoi(env_bn) : 128);
+    const int max_bn = env_bn ? atoi(env_bn) : 256;
     const char* env_st = getenv("WS_TC2_MAX_STAGES");
     const int max_st = env_st ? atoi(env_st) : WS_TC_MAX_STAGES;
     for (int pass = 0; pass < 2 && bn == 0; ++pass)
         for (int ci = 0; ci < 4; ++ci) {
             const int c = cands[ci];
-            if (s.Cout % c != 0 || c > max_bn) continue;
+            if (s.Cout % c != 0 || c > max_bn || (c == 256 && (!wide_ok || pass == 1))) continue;
             const int wrows = c / cl;            // clusters: each CTA fetches (and multicasts) bn / cl weight rows
             if ((wrows * q->bk_bytes) % 1024 != 0) continue;   // ... a whole number of 1024-B swizzle atoms
-            const int staging = nstage_bufs * 128 * c * es + 3 * c * 4 + WS_TC_EPI_SCRATCH;
+            const int staging = nstage_bufs * 128 * std::min(c, 128) * es + 3 * c * 4 + WS_TC_EPI_SCRATCH;
             const int stage_bytes = (128 + c) * q->bk_bytes;
             const int n = (budget - staging) / stage_bytes;
             if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > max_st ? max_st : n; break; }
@@ -315,7 +331,6 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     if (bn == 0) { *unsupported = true; return false; }
     q->bn = bn; q->nstages = nst;
     q->tiles_n = s.Cout / bn;
-    const int mtiles = q->tiles_t * q->tiles_f * q->tiles_b;
     q->num_tiles = q->tiles_n * ((mtiles + cl - 1) / cl);
     q->panel_bytes = bn * es >= 128 ? 128 : bn * es;
     const int panel_cols = q->panel_bytes / es;
@@ -363,20 +378,13 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     }
     for (; oi < 4; ++oi) q->omap[oi] = q->omap[0];
     if (!q->has_epin) q->imap = q->omap[0];
-    const int g_num_sms = ws_num_sms();
     q->cl = cl;
-    if (pair) {
-        int ncl = ws_tc3_max_clusters(cl);
-        if (ncl <= 0) ncl = g_num_sms / cl;
-        q->grid = cl * (q->num_tiles < ncl ? q->num_tiles : ncl);
-    } else {
-        q->grid = q->num_tiles < g_num_sms ? q->num_tiles : g_num_sms;
-    }
-    q->smem_bytes = nst * (128 + bn) * q->bk_bytes + nstage_bufs * 128 * bn * es + 3 * bn * 4 + WS_TC_EPI_SCRATCH + 1024;
-    q->epi = e;
+    if (pair) q->grid = cl * (q->num_tiles < ncl ? q->num_tiles : ncl);
+    else q->grid = q->num_tiles < g_num_sms ? q->num_tiles : g_num_sms;
+    q->smem_bytes = nst * (128 + bn) * q->bk_bytes + nstage_bufs * 128 * std::min(bn, 128) * es + 3 * bn * 4 +
+                    WS_TC_EPI_SCRATCH + 1024;
     const char* env_sh = getenv("WS_TC2_SHIFT_TEST");
     q->dbg_shift = env_sh ? atoi(env_sh) : -1;
-    { const char* eg = getenv("WS_EPI_GENERIC"); q->epi_generic = eg != nullptr && atoi(eg) != 0; }
     return true;
 }
 

@@ -5,6 +5,11 @@
 //   * persistent CTAs (one per SM) walking a static tile schedule; the TMA producer runs ahead into the next tile's
 //     operands while the consumers finish the current tile's epilogue;
 //   * bn up to 128: each of the two consumer warpgroups keeps a 64 x bn fp32 accumulator in registers;
+//   * BN = 256 (16-bit activations, lean epilogue, no epilogue-input tile): 128 x 256 tiles, which halve the A-operand
+//     reads (L2 and shared memory) and the epilogue passes per FLOP.  The accumulator is 128 fp32 per consumer thread, so the producer warpgroup gives registers back
+//     (setmaxnreg 40) and the consumers take them (232); wgmma N and dtype are compile-time (m64n256k16, four per
+//     128-byte k-block); the output tile goes through one 128-column staging buffer in two passes, so that three ring
+//     stages still fit;
 //   * coalesced, asynchronous epilogue: per-channel parameters staged in smem, residual / Res2 "add2" tiles fetched by
 //     TMA into swizzled smem while the mainloop runs, outputs packed into 128-B-swizzled smem panels and written with
 //     TMA stores (cp.async.bulk.tensor ... bulk_group), which also clips out-of-range rows/positions for free;
@@ -46,8 +51,11 @@ __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* 
         : "memory");
 }
 
-template <int KIND, int LEAN, int CL>
+// BN = 0: N tile p.bn <= 128 chosen at run time.  BN = 256: the wide 16-bit variant (p.bn == 256, p.bk_bytes == 128).
+template <int KIND, int LEAN, int CL, int BN>
 __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __grid_constant__ WsTc2Params p) {
+    static_assert(BN == 0 || (BN == 256 && KIND == 1 && (LEAN == WS_BF16 + 1 || LEAN == WS_F16 + 1)), "wide tile: lean 16-bit");
+    constexpr int NPASS = BN == 256 ? 2 : 1;             // staging passes per output tile
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_bar[2 * WS_TC_MAX_STAGES + 2];
 
@@ -58,8 +66,9 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
     const int es = KIND == 0 ? 4 : 2;
     const int panel_bytes = p.panel_bytes;               // row bytes of one staging panel (128 / 64)
     const int panel_cols = panel_bytes / es;
-    const int npanels = p.bn / panel_cols;
-    const int tile_out_bytes = 128 * p.bn * es;          // one full output tile in staging
+    const int pass_cols = BN == 256 ? 128 : p.bn;        // output columns staged per pass
+    const int npanels = pass_cols / panel_cols;
+    const int tile_out_bytes = 128 * pass_cols * es;     // one staging pass of one output tile
     const uint32_t ring = base;
     const uint32_t stg_out = ring + (uint32_t)(p.nstages * stage_bytes);                  // p.nout output tiles
     const uint32_t stg_in = stg_out + (uint32_t)(p.nout * tile_out_bytes);                // only if p.has_epin
@@ -96,9 +105,10 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
     __syncthreads();
     if constexpr (CL > 1) cluster_sync();   // the peers' barriers are initialised before any multicast or remote arrive
 
-    if (warp == 0) {
+    if (warp < 4) {
+        if constexpr (BN == 256) ws_wg::setmaxnreg_dec<40>();   // 128 x 40 + 256 x 232 <= 64 K registers
         // ================================ TMA producer ================================
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             const int bk_elems = p.bk_bytes / es;
             const int wrows = p.bn / CL;             // weight rows this CTA fetches (and multicasts) per k-block
             int it = 0, j = 0;
@@ -139,7 +149,8 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
                 }
             }
         }
-    } else if (warp >= 4) {
+    } else {
+        if constexpr (BN == 256) ws_wg::setmaxnreg_inc<232>();
         // ================================ consumers: mainloop + epilogue ================================
         const int wg = (warp - 4) >> 2;                  // accumulator rows [64 wg, 64 wg + 64) of the tile
         const int et = threadIdx.x - 128;                // 0..255
@@ -161,7 +172,7 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
         for (int tile = cid; tile < p.num_tiles; tile += ncl, ++j) {
             int n0, t0, f0, b0;
             decode(tile, n0, t0, f0, b0);
-            float acc[64];
+            float acc[BN == 256 ? 128 : 64];
             const int nkit = p.nk_total * p.nsplit;
             int prev = -1;
             for (int kit = 0; kit < nkit; ++kit) {
@@ -172,8 +183,14 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
                     adesc = ws_wg::desc(sa + (uint32_t)p.bk_bytes, p.bk_bytes) | ((uint64_t)(p.dbg_shift & 7) << 49);
                 const uint64_t bdesc = ws_wg::desc(ring + (uint32_t)(s * stage_bytes + a_bytes), p.bk_bytes);
                 ws_wg::fence();
-                for (int k = 0; k < kper; ++k)
-                    ws_wg::mma_n(p.bn, dt, acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kit | k) != 0));
+                if constexpr (BN == 256) {
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+                        ws_wg::mma16_n256<LEAN - 1>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kit | k) != 0));
+                } else {
+                    for (int k = 0; k < kper; ++k)
+                        ws_wg::mma_n(p.bn, dt, acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kit | k) != 0));
+                }
                 ws_wg::commit();
                 ws_wg::wait<1>();
                 if (prev >= 0) release(prev);
@@ -181,16 +198,9 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
                 if (++s == p.nstages) { s = 0; ph ^= 1u; }
             }
             ws_wg::wait<0>();
-            ws_wg::fence_regs<64>(acc);
+            ws_wg::fence_regs<BN == 256 ? 128 : 64>(acc);
             if (prev >= 0) release(prev);
 
-            // staging buffers are free once the previous tile's TMA stores have finished reading them
-            if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            if (n0 != last_n0) {
-                epi_stage_params(p, spar, n0, et);
-                last_n0 = n0;
-            }
-            epi_bar_sync();
             // row -> output position (for the per-row epilogue inputs that are not tile-shaped)
             const int t = t0 + (r & ((1 << p.bt_log2) - 1));
             const int f = f0 + ((r >> p.bt_log2) & ((1 << p.bf_log2) - 1));
@@ -202,31 +212,43 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
                 eb = (int)(pos / e.FT);
                 etm = (int)(pos % e.T);
             }
-            if (p.has_epin) mbar_wait(bar_ifull, (uint32_t)j & 1u);
-            const EpiTile xt{spar, stg_in, stg_out, tile_out_bytes, panel_bytes, panel_cols, n0, r, valid, eb, etm};
-            // 64-column blocks of the accumulator: lanes 0..15 take columns [0, 32) of their row, lanes 16..31 [32, 64)
 #pragma unroll
-            for (int cb = 0; cb < 2; ++cb) {
-                if (cb * 64 < p.bn) {
-                    uint32_t raw[32];
-                    ws_wg::frag_to_rows<64>(acc, cb * 64, scr, reinterpret_cast<float*>(raw));
-                    const int c = cb * 64 + (lane >> 4) * 32;
-                    if (c < p.bn) epi_chunk<LEAN>(p, xt, raw, c);
+            for (int h = 0; h < NPASS; ++h) {
+                const int hc = h * 128;                      // first tile column of this staging pass
+                // staging buffers are free once the previous TMA stores (previous tile or pass) have finished reading them
+                if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                if (h == 0 && n0 != last_n0) {
+                    epi_stage_params(p, spar, n0, et);
+                    last_n0 = n0;
                 }
+                epi_bar_sync();
+                if (p.has_epin) mbar_wait(bar_ifull, (uint32_t)j & 1u);
+                // the pass's columns [hc, hc + pass_cols) are columns [0, pass_cols) of the staging buffer
+                const EpiTile xt{spar + hc, stg_in, stg_out, tile_out_bytes, panel_bytes, panel_cols, n0 + hc, r, valid, eb, etm};
+                // 64-column blocks of the accumulator: lanes 0..15 take columns [0, 32) of their row, lanes 16..31 [32, 64)
+#pragma unroll
+                for (int cb = 0; cb < 2; ++cb) {
+                    if (cb * 64 < pass_cols) {
+                        uint32_t raw[32];
+                        ws_wg::frag_to_rows<64>(acc, hc + cb * 64, scr, reinterpret_cast<float*>(raw));
+                        const int c = cb * 64 + (lane >> 4) * 32;
+                        if (c < pass_cols) epi_chunk<LEAN>(p, xt, raw, c);
+                    }
+                }
+                // the epilogue-input tile is drained: hand it back
+                __syncwarp();
+                if (lane == 0 && p.has_epin) mbar_arrive(bar_iempty);
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                epi_bar_sync();
+                if (et == 0) {
+                    for (int o = 0; o < p.nout; ++o)
+                        for (int pn = 0; pn < npanels; ++pn)
+                            tma_store_4d(&p.omap[o], stg_out + (uint32_t)(o * tile_out_bytes + pn * 128 * panel_bytes),
+                                         n0 + hc + pn * panel_cols, t0, f0, b0);
+                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                }
+                if constexpr (LEAN == WS_BF16 + 1 || LEAN == WS_F16 + 1) epi_colsum<LEAN>(p, stg_out, et, n0 + hc, pass_cols, t0, b0);
             }
-            // the epilogue-input tile is drained: hand it back
-            __syncwarp();
-            if (lane == 0 && p.has_epin) mbar_arrive(bar_iempty);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            epi_bar_sync();
-            if (et == 0) {
-                for (int o = 0; o < p.nout; ++o)
-                    for (int pn = 0; pn < npanels; ++pn)
-                        tma_store_4d(&p.omap[o], stg_out + (uint32_t)(o * tile_out_bytes + pn * 128 * panel_bytes),
-                                     n0 + pn * panel_cols, t0, f0, b0);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-            if constexpr (LEAN == WS_BF16 + 1 || LEAN == WS_F16 + 1) epi_colsum<LEAN>(p, stg_out, et, n0, t0, b0);
         }
         if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
@@ -237,9 +259,9 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
 }  // namespace
 
 namespace {
-template <int KIND, int LEAN, int CL>
+template <int KIND, int LEAN, int CL, int BN = 0>
 inline cudaError_t tc2_attr1() {
-    return cudaFuncSetAttribute(ws_conv_gemm_tc2_kernel<KIND, LEAN, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem2);
+    return cudaFuncSetAttribute(ws_conv_gemm_tc2_kernel<KIND, LEAN, CL, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem2);
 }
 template <int CL>
 inline cudaError_t tc2_attr() {
@@ -248,12 +270,14 @@ inline cudaError_t tc2_attr() {
     if (e == cudaSuccess) e = tc2_attr1<0, WS_F32 + 1, CL>();
     if (e == cudaSuccess) e = tc2_attr1<1, WS_BF16 + 1, CL>();
     if (e == cudaSuccess) e = tc2_attr1<1, WS_F16 + 1, CL>();
+    if (e == cudaSuccess) e = tc2_attr1<1, WS_BF16 + 1, CL, 256>();
+    if (e == cudaSuccess) e = tc2_attr1<1, WS_F16 + 1, CL, 256>();
     return e;
 }
-template <int KIND, int LEAN, int CL>
+template <int KIND, int LEAN, int CL, int BN = 0>
 inline cudaError_t tc2_go(const WsTc2Params* p, cudaStream_t s) {
     if constexpr (CL == 1) {
-        ws_conv_gemm_tc2_kernel<KIND, LEAN, 1><<<p->grid, kThreads2, p->smem_bytes, s>>>(*p);
+        ws_conv_gemm_tc2_kernel<KIND, LEAN, 1, BN><<<p->grid, kThreads2, p->smem_bytes, s>>>(*p);
         return cudaGetLastError();
     } else {
         cudaLaunchConfig_t cfg = {};
@@ -262,11 +286,12 @@ inline cudaError_t tc2_go(const WsTc2Params* p, cudaStream_t s) {
         at.id = cudaLaunchAttributeClusterDimension;
         at.val.clusterDim.x = CL; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
         cfg.attrs = &at; cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, ws_conv_gemm_tc2_kernel<KIND, LEAN, CL>, *p);
+        return cudaLaunchKernelEx(&cfg, ws_conv_gemm_tc2_kernel<KIND, LEAN, CL, BN>, *p);
     }
 }
 template <int CL>
 inline cudaError_t tc2_dispatch(const WsTc2Params* p, cudaStream_t s, int lean) {
+    if (p->bn == 256) return lean == WS_BF16 + 1 ? tc2_go<1, WS_BF16 + 1, CL, 256>(p, s) : tc2_go<1, WS_F16 + 1, CL, 256>(p, s);
     if (lean == WS_F32 + 1) return tc2_go<0, WS_F32 + 1, CL>(p, s);
     if (lean == WS_BF16 + 1) return tc2_go<1, WS_BF16 + 1, CL>(p, s);
     if (lean == WS_F16 + 1) return tc2_go<1, WS_F16 + 1, CL>(p, s);
@@ -318,16 +343,24 @@ extern "C" int ws_tc3_max_clusters(int cl) {
     at.val.clusterDim.x = (unsigned)cl; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
     cfg.attrs = &at; cfg.numAttrs = 1;
     int n = 0;
-    cudaError_t e = cl == 4 ? cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 4>, &cfg)
-                            : cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 2>, &cfg);
+    cudaError_t e = cl == 4 ? cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 4, 0>, &cfg)
+                            : cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 2, 0>, &cfg);
     if (e != cudaSuccess) { cudaGetLastError(); n = 0; }
     cache[dev][k] = n; have[dev][k] = true;
     return n;
 }
 
+// the 256-wide instantiation has the lean 16-bit epilogue only and no room for an epilogue-input tile
+static const char* ws_tc2_wide_check(const WsTc2Params* p, int lean) {
+    if (p->bn == 256 && ((lean != WS_BF16 + 1 && lean != WS_F16 + 1) || p->has_epin || p->bk_bytes != 128))
+        return "conv: 256-wide tiles need the lean 16-bit epilogue, 128-byte k-blocks and no residual / add2 tile";
+    return nullptr;
+}
+
 extern "C" const char* ws_tc2_launch(const WsTc2Params* p, cudaStream_t s) {
     const int lean = p->epi_generic ? 0 : ws_tc_lean_kind(p);
     if (const char* m = ws_tc_colsum_check(p, lean)) return m;
+    if (const char* m = ws_tc2_wide_check(p, lean)) return m;
     const cudaError_t e = tc2_dispatch<1>(p, s, lean);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
@@ -335,6 +368,7 @@ extern "C" const char* ws_tc2_launch(const WsTc2Params* p, cudaStream_t s) {
 extern "C" const char* ws_tc3_launch(const WsTc2Params* p, cudaStream_t s) {
     const int lean = p->epi_generic ? 0 : ws_tc_lean_kind(p);
     if (const char* m = ws_tc_colsum_check(p, lean)) return m;
+    if (const char* m = ws_tc2_wide_check(p, lean)) return m;
     if (p->cl != 2 && p->cl != 4) return "ws_tc3_launch: cluster size must be 2 or 4";
     const cudaError_t e = p->cl == 4 ? tc2_dispatch<4>(p, s, lean) : tc2_dispatch<2>(p, s, lean);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);

@@ -287,12 +287,12 @@ __device__ __forceinline__ void epi_chunk(const WsTc2Params& p, const EpiTile& x
 }
 
 // fused SE squeeze (WsEpi::colsum): column sums of the staged (already rounded) tile, read back from the swizzled staging
-// panels while the TMA store drains them; thread = (column pair, 64-row half), pairs past the tile's bn columns idle.
-// 16-bit lean instantiations only.
+// panels while the TMA store drains them; thread = (column pair, 64-row half), pairs past the ncols staged columns (the
+// tile's bn, or one 128-column pass of a 256-wide tile, whose first channel is n0) idle.  16-bit lean instantiations only.
 template <int LEAN>
-__device__ __forceinline__ void epi_colsum(const WsTc2Params& p, uint32_t stg_out, int et, int n0, int t0, int b0) {
+__device__ __forceinline__ void epi_colsum(const WsTc2Params& p, uint32_t stg_out, int et, int n0, int ncols, int t0, int b0) {
     const WsEpi& e = p.epi;
-    if (e.colsum != nullptr && 2 * (et & 127) < p.bn && b0 < p.B && t0 + (et >> 7) * 64 < p.T) {   // units past the last position do not exist
+    if (e.colsum != nullptr && 2 * (et & 127) < ncols && b0 < p.B && t0 + (et >> 7) * 64 < p.T) {   // units past the last position do not exist
         const int cpair = et & 127, rh = et >> 7;
         const int pos0 = t0 + rh * 64;
         const int nvalid = min(64, p.T - pos0);

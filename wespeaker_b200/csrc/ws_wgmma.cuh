@@ -121,6 +121,35 @@ __device__ __forceinline__ void mma_n(int n, int dt, float* d, uint64_t da, uint
     else mma<16>(dt, d, da, db, acc);
 }
 
+// m64n256k16 with the 16-bit operand type fixed at compile time (DT: 1 bf16, 2 fp16): 128 accumulator registers per thread
+#define WS_WG_REGS_N256                                                                                                     \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "  \
+    "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "    \
+    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, "    \
+    "%71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, "    \
+    "%94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, "     \
+    "%114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define WS_WG_OPS_N256                                                                                                       \
+    WS_WG_F8(0), WS_WG_F8(8), WS_WG_F8(16), WS_WG_F8(24), WS_WG_F8(32), WS_WG_F8(40), WS_WG_F8(48), WS_WG_F8(56),          \
+        WS_WG_F8(64), WS_WG_F8(72), WS_WG_F8(80), WS_WG_F8(88), WS_WG_F8(96), WS_WG_F8(104), WS_WG_F8(112), WS_WG_F8(120)
+template <int DT>
+__device__ __forceinline__ void mma16_n256(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    static_assert(DT == 1 || DT == 2, "16-bit wgmma");
+    if constexpr (DT == 1)
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+                     WS_WG_REGS_N256 ", %128, %129, p, 1, 1, 0, 0;\n\t}" : WS_WG_OPS_N256 : "l"(da), "l"(db), "r"(acc));
+    else
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\twgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+                     WS_WG_REGS_N256 ", %128, %129, p, 1, 1, 0, 0;\n\t}" : WS_WG_OPS_N256 : "l"(da), "l"(db), "r"(acc));
+}
+
+// per-thread register budget of the executing warpgroup (all four warps execute it): the producer warpgroup hands
+// registers back to the CTA's pool, the consumer warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // Row-wise access to an accumulator for epilogues written per output row: the warp's 16 rows x NC columns (NC = 64, 32 or
 // 16 starting at column c0 of the fragment) go through a per-warp shared-memory scratch of 16 x kScrPitch floats, after
 // which lane l owns row (l & 15) and the NC/2 consecutive columns starting at (l >> 4) * NC/2.
