@@ -304,12 +304,17 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     }
     // rounds of the persistent schedule: tiles of bn columns over ncl clusters
     auto rounds = [&](int c) { return ((long long)(s.Cout / c) * ((mtiles + cl - 1) / cl) + ncl - 1) / ncl; };
-    // 256-wide tiles (16-bit, lean epilogue, no epilogue-input tile, 128-byte k-blocks; one 128-column staging buffer)
-    // halve the A-operand reads and the epilogue passes per FLOP, but a tile is twice the work: taken when the schedule
-    // then needs at most 10 % more time than with 128-wide tiles, counted in 128-wide rounds (20 r256 <= 11 r128)
+    // 256-wide tiles (16-bit, lean epilogue without row bias, no epilogue-input tile, 128-byte k-blocks) halve the
+    // A-operand reads and the epilogue passes per FLOP, but a tile is twice the work: taken when the schedule then needs
+    // at most 10 % more time than with 128-wide tiles, counted in 128-wide rounds (20 r256 <= 11 r128)
     q->epi = e; q->bn = 256; q->panel_bytes = 128;
     const bool wide_ok = s.Cout % 256 == 0 && q->kind == 1 && !q->has_epin && q->bk_bytes == 128 && !q->epi_generic &&
-                         ws_tc_lean_kind(q) == s.dt + 1 && 20 * rounds(256) <= 11 * rounds(128);
+                         ws_tc_lean_kind(q) == s.dt + 1 && e.rowbias == nullptr && 20 * rounds(256) <= 11 * rounds(128);
+    // staging + per-channel parameters (+ the row-wise epilogue's scratch): the 256-wide tile stages its whole output
+    // tile at once and double-buffers its parameters, and its epilogue works in fragment layout without scratch
+    auto staging_bytes = [&](int c) {
+        return c == 256 ? 128 * c * es + 2 * 3 * c * 4 : nstage_bufs * 128 * c * es + 3 * c * 4 + WS_TC_EPI_SCRATCH;
+    };
     // widest N tile whose staging + >=3 ring stages fit (>=2 accepted as a last resort, never for 256)
     int bn = 0, nst = 0;
     const int cands[4] = {256, 128, 64, 32};
@@ -323,7 +328,7 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
             if (s.Cout % c != 0 || c > max_bn || (c == 256 && (!wide_ok || pass == 1))) continue;
             const int wrows = c / cl;            // clusters: each CTA fetches (and multicasts) bn / cl weight rows
             if ((wrows * q->bk_bytes) % 1024 != 0) continue;   // ... a whole number of 1024-B swizzle atoms
-            const int staging = nstage_bufs * 128 * std::min(c, 128) * es + 3 * c * 4 + WS_TC_EPI_SCRATCH;
+            const int staging = staging_bytes(c);
             const int stage_bytes = (128 + c) * q->bk_bytes;
             const int n = (budget - staging) / stage_bytes;
             if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > max_st ? max_st : n; break; }
@@ -381,8 +386,7 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     q->cl = cl;
     if (pair) q->grid = cl * (q->num_tiles < ncl ? q->num_tiles : ncl);
     else q->grid = q->num_tiles < g_num_sms ? q->num_tiles : g_num_sms;
-    q->smem_bytes = nst * (128 + bn) * q->bk_bytes + nstage_bufs * 128 * std::min(bn, 128) * es + 3 * bn * 4 +
-                    WS_TC_EPI_SCRATCH + 1024;
+    q->smem_bytes = nst * (128 + bn) * q->bk_bytes + staging_bytes(bn) + 1024;
     const char* env_sh = getenv("WS_TC2_SHIFT_TEST");
     q->dbg_shift = env_sh ? atoi(env_sh) : -1;
     return true;

@@ -143,6 +143,14 @@ __device__ __forceinline__ void epi_stage_params(const WsTc2Params& p, float* sp
     }
 }
 
+// tanh for 16-bit outputs: tanh(x) = 1 - 2 / (e^{2x} + 1) on ex2.approx + rcp.approx (abs error ~1e-7, far below the
+// output rounding), 5 instructions per element instead of the ~25 of tanhf
+__device__ __forceinline__ float tanh16(float x) {
+    float ex;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(x * 2.885390081777927f));
+    return 1.f - __fdividef(2.f, ex + 1.f);
+}
+
 // LEAN != 0 (= WsDType of the activations + 1) compiles only the common epilogue: bias, ReLU, BN scale/shift, residual
 // tile, ReLU, one output (+ its 3xTF32 low twin for fp32).  The generic epilogue (row bias, gates, Res2 second output,
 // tanh/sigmoid, every dtype) is ~100 KB of SASS of which a given layer executes a few KB scattered between never-taken
@@ -178,14 +186,8 @@ __device__ __forceinline__ void epi_chunk(const WsTc2Params& p, const EpiTile& x
             if constexpr (DT == WS_F32) {
                 ws_act_vec<32>(v, WS_ACT_TANH);
             } else {
-                // 16-bit outputs: tanh(x) = 1 - 2 / (e^{2x} + 1) on ex2.approx + rcp.approx (abs error ~1e-7, far below
-                // the output rounding), 5 instructions per element instead of the ~25 of tanhf
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float ex;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(v[i] * 2.885390081777927f));
-                    v[i] = 1.f - __fdividef(2.f, ex + 1.f);
-                }
+                for (int i = 0; i < 32; ++i) v[i] = tanh16(v[i]);
             }
         }
         if (e.scale != nullptr) {
@@ -287,8 +289,8 @@ __device__ __forceinline__ void epi_chunk(const WsTc2Params& p, const EpiTile& x
 }
 
 // fused SE squeeze (WsEpi::colsum): column sums of the staged (already rounded) tile, read back from the swizzled staging
-// panels while the TMA store drains them; thread = (column pair, 64-row half), pairs past the ncols staged columns (the
-// tile's bn, or one 128-column pass of a 256-wide tile, whose first channel is n0) idle.  16-bit lean instantiations only.
+// panels while the TMA store drains them; thread = (column pair, 64-row half), pairs past the tile's ncols = bn <= 128
+// columns idle.  16-bit lean instantiations only (the 256-wide tile sums on its helper warps, ws_gemm_tc2.cu).
 template <int LEAN>
 __device__ __forceinline__ void epi_colsum(const WsTc2Params& p, uint32_t stg_out, int et, int n0, int ncols, int t0, int b0) {
     const WsEpi& e = p.epi;
