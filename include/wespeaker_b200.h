@@ -40,8 +40,8 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
  * returns an error on such an engine. */
 int ws_engine_create_plan_check(const char* model_name, const char* precision, int feat_dim, int embed_dim, ws_engine** out);
 /* options: "two_emb_layer", "emb_bn" (model_args), "cuda_graph" (default 1), "force_simt" (debug cross-check),
- * "tc_version" (1: one-tile-per-CTA tensor-core kernel, 2: persistent / TMA-store kernel, 3 (default): + weight-sharing CTA clusters
- * on the large layers),
+ * "tc_version" (2: persistent / TMA-store tensor-core kernel, 3 (default): + weight-sharing CTA clusters on the large layers;
+ * any other value is an error),
  * "res2_fused" (default 1: ECAPA Res2 chains run as one fused persistent kernel per stage for 16-bit precisions) */
 int ws_engine_set_option(ws_engine* e, const char* key, long long value);
 /* one reference state_dict entry (fp32 host data, reference key names, SURVEY.md Appendix C). */
@@ -141,7 +141,9 @@ typedef struct {
     void* out;                /* [B][Fo][To][out_ld] */
     long long out_ld;
     int dtype;                /* 0 fp32 (tf32 MMA when use_tc), 1 bf16, 2 fp16 */
-    int use_tc;               /* 0: fp32 FFMA kernel, 1: tensor-core v1, 2: persistent v2, 3: v2 with weight-sharing clusters */
+    int use_tc;               /* 0: fp32 FFMA kernel, 2: persistent tensor-core kernel, 3: the same with weight-sharing clusters on
+                                 large layers, 4: 3 with 3x3 convs on the halo-resident 3x3 kernel where it applies; 1 is an
+                                 error */
     /* 3xTF32 (dtype 0, use_tc 2): low parts v - tf32_trunc(v) of x and w (inputs) and of out (written); all NULL = off */
     const void* x_lo;
     const void* w_lo;

@@ -77,7 +77,7 @@ def run_conv(x_cl, w, bias, scale, shift, res, prec, use_tc, kf, kt, dil, pad, s
         r = res.to(DEV, tdt).contiguous()
         keep.append(r)
         d.res, d.res_ld = r.data_ptr(), Cout
-    d.act1, d.act2, d.out, d.out_ld, d.dtype, d.use_tc = act1, act2, out.data_ptr(), Cout, code, int(use_tc)  # 0 FFMA, 1 tc v1, 2 tc v2
+    d.act1, d.act2, d.out, d.out_ld, d.dtype, d.use_tc = act1, act2, out.data_ptr(), Cout, code, int(use_tc)  # 0 FFMA, 2 tc, 3 tc + clusters
     if prec == "tf32x3":
         xl, wl = tf32_lo(xd).contiguous(), tf32_lo(wp).contiguous()
         out_lo = torch.zeros_like(out)
@@ -121,12 +121,16 @@ CONV_CASES = [
     ("k3_d2_128_32", 2, 1, 100, 128, 32, 1, 3, (1, 2), (0, 2), (1, 1)),
     ("pw_1536_nores", 2, 1, 200, 256, 1536, 1, 1, (1, 1), (0, 0), (1, 1)),
     ("pw_many_tiles", 64, 1, 200, 128, 512, 1, 1, (1, 1), (0, 0), (1, 1)),
+    ("pw_1504_nores", 2, 1, 150, 512, 1504, 1, 1, (1, 1), (0, 0), (1, 1)),   # XVEC's padded width: 47 tiles of 32 channels
+    ("k3_d4_c96", 3, 1, 80, 96, 96, 1, 3, (1, 4), (0, 4), (1, 1)),          # 3 tiles of 32 channels, ragged 16-bit k-blocks
+    ("pw_c160_ragged", 2, 1, 130, 160, 256, 1, 1, (1, 1), (0, 0), (1, 1)),  # one ragged k-block of a 1x1 conv
+    ("c3x3_dil_f2", 2, 12, 30, 64, 64, 3, 3, (2, 1), (2, 1), (1, 1)),      # dilated along F: 2-D position tiles
 ]
 
 
 @pytest.mark.parametrize("case", CONV_CASES, ids=[c[0] for c in CONV_CASES])
-@pytest.mark.parametrize("mode", ["fp32-simt", "tf32-tc", "bf16-tc", "fp16-tc", "bf16-simt", "tf32-tc2", "bf16-tc2", "fp16-tc2",
-                                  "tf32x3-tc2", "bf16-tc3", "tf32-tc3", "fp16-tc3", "tf32x3-tc3"])
+@pytest.mark.parametrize("mode", ["fp32-simt", "bf16-simt", "tf32-tc2", "bf16-tc2", "fp16-tc2", "tf32x3-tc2", "bf16-tc3", "tf32-tc3",
+                                  "fp16-tc3", "tf32x3-tc3"])
 def test_conv_operator(case, mode):
     name, B, F, T, Cin, Cout, kf, kt, dil, pad, stride = case
     prec, path = mode.split("-")
@@ -142,7 +146,7 @@ def test_conv_operator(case, mode):
     if path == "tc3":
         os.environ["WS_TC3_MIN_POS"] = "1"   # force the cluster kernel on these small shapes (odd tile tails included)
     try:
-        out = run_conv(x, w, bias, scale, shift, res, prec, {"simt": 0, "tc": 1, "tc2": 2, "tc3": 3}[path], kf, kt, dil, pad,
+        out = run_conv(x, w, bias, scale, shift, res, prec, {"simt": 0, "tc2": 2, "tc3": 3}[path], kf, kt, dil, pad,
                        stride, 1, 1)
     finally:
         os.environ.pop("WS_TC3_MIN_POS", None)
@@ -496,19 +500,6 @@ def test_model_tf32x3_tensor_cores_meet_fp32_bar(key):
     rel = rel_l2(emb, G_MODELS[key])
     print(f"{key} tf32x3: rel-L2 max {rel.max():.3e}")
     assert rel.max() <= 1e-4, (key, rel)
-
-
-def test_tc_v1_kernel_still_matches():
-    """The one-tile-per-CTA tensor-core kernel (tc_version=1) stays available as a cross-check of the persistent one."""
-    key = "ECAPA_TDNN_c512__s0_B4_T198"
-    name, seed, B, T = parse_case(key)
-    feats = torch.from_numpy(syn.make_feats(B, T, 80, seed=seed + 17 * T)).to(DEV)
-    m1 = from_synthetic(name, seed, precision="bf16")
-    m1.set_option("tc_version", 1)
-    m2 = from_synthetic(name, seed, precision="bf16")
-    e1, e2 = m1.embed(feats).cpu().numpy(), m2.embed(feats).cpu().numpy()
-    assert rel_l2(e1, G_MODELS[key]).max() <= 1e-2 and rel_l2(e2, G_MODELS[key]).max() <= 1e-2
-    assert rel_l2(e1, e2).max() <= 2e-2
 
 
 @pytest.mark.parametrize("prec", ["tf32", "bf16", "fp16"])

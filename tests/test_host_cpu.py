@@ -239,6 +239,28 @@ def test_plan_check_reports_missing_and_misshaped_tensors_and_never_computes():
         L.ws_engine_destroy(h)
 
 
+def test_tc_version_selects_the_persistent_kernel_and_refuses_1():
+    """tc_version 2 puts every tensor-core conv on the persistent kernel, 3 (the default) adds weight-sharing clusters on the
+    large layers.  1 named the one-tile-per-CTA kernel, which is gone: the option and ws_conv's use_tc = 1 are errors."""
+    import ctypes as C
+    labels = {}
+    for v in (2, 3):
+        m = from_synthetic("ECAPA_TDNN_c512", precision="bf16")
+        m.set_option("tc_version", v)
+        labels[v] = [n for n, _ in m.plan_check(128, 200)]
+    assert any(n.startswith("conv_tc2") for n in labels[2]) and not any(n.startswith("conv_tc3") for n in labels[2])
+    assert any(n.startswith("conv_tc3") for n in labels[3])
+    m = from_synthetic("ECAPA_TDNN_c512", precision="bf16")
+    m.set_option("tc_version", 1)
+    with pytest.raises(lib.B200Error, match="one-tile-per-CTA"):
+        m.plan_check(2, 200)
+    L = lib.load()
+    d = lib.ConvDesc()
+    d.use_tc = 1
+    assert L.ws_conv(C.byref(d), None) != 0
+    assert b"one-tile-per-CTA" in L.ws_last_error()
+
+
 @pytest.mark.parametrize("name,prec,B,T", [("ResNet34", "fp16", 2, 99), ("ResNet34", "tf32x3", 1, 40), ("ResNet50", "bf16", 1, 64),
                                           ("XVEC", "bf16", 2, 40)])
 def test_plan_arithmetic_matches_oracle_on_the_host(name, prec, B, T, tmp_path):

@@ -42,7 +42,6 @@ if __name__ == "__main__":
         B, T, ci, co, k, d = shapes[name]
         for tcv in (2, 3):
             for knobs in ({}, {"WS_TC2_MAX_BN": "128"}):
-                if tcv == 1 and any(kk.startswith("WS_TC2") for kk in knobs): continue
                 if k == 1 and "WS_TILE_BT" in knobs: continue
                 for kk in ("WS_TILE_BT", "WS_TC2_MAX_STAGES", "WS_TC2_MAX_BN"): os.environ.pop(kk, None)
                 os.environ.update(knobs)

@@ -58,7 +58,7 @@ def cases():
             out.append((name, prec, 2, 200, False, {"two_emb_layer": True}, {}))
     for prec in ("tf32x3", "bf16"):
         out.append(("ECAPA_TDNN_c512", prec, 2, 200, False, {"emb_bn": True}, {}))
-    for opts in ({"force_simt": 1}, {"tc_version": 1}, {"tc_version": 2}):
+    for opts in ({"force_simt": 1}, {"tc_version": 2}):
         for prec in ("tf32x3", "bf16"):
             out.append(("ResNet34", prec, 2, 200, False, {}, opts))
     return out

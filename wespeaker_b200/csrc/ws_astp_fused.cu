@@ -29,13 +29,6 @@ constexpr int kXTileBytes = 128 * 256;   // 128 frames x 128 channels of x, row 
 constexpr int kXSlots = 3;
 constexpr int kSmemA = 2 * kHPanelBytes + 2 * 2 * kWPanelBytes + kXSlots * kXTileBytes + 1024;   // H chunk + two W2 blocks + x ring
 
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-            "r"(dst),
-        "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 __device__ __forceinline__ float ex2f(float v) {
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));

@@ -32,18 +32,6 @@ constexpr int kHPad = 8;                     // zero rows in front of t = 0 (>= 
 constexpr int kMaxSeg = 6;
 constexpr int kParamFloats = 1024 + 1024 + 128 + 1536 + kMaxSeg * 128 + kMaxSeg * 64 + kMaxSeg * 32;
 
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-            "r"(dst),
-        "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map),
-                 "r"(src), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
 template <int DT>
 __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __grid_constant__ WsCamParams p) {
     extern __shared__ uint8_t smem_raw[];

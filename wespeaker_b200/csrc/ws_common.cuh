@@ -281,25 +281,12 @@ struct WsSimtParams {
 #define WS_TC_MAX_STAGES 8
 // per-warp accumulator scratch of the row-wise GEMM epilogues (ws_wgmma.cuh, frag_to_rows): 8 consumer warps x 16 x 68 floats
 #define WS_TC_EPI_SCRATCH (8 * 16 * 68 * 4)
+// one tap of the tensor-core conv: source map, first channel, time / frequency offset, first weight column, k-blocks
 struct WsTcTap {
     int map, c0, dt, df, wk, nkb;
 };
-struct WsTcParams {
-    CUtensorMap amap[WS_MAX_SRC];
-    CUtensorMap wmap;
-    WsTcTap taps[WS_MAX_TAPS];
-    int ntaps, nk_total;
-    int bk_bytes;                       // 128 / 64 / 32 : k-block row bytes == TMA / wgmma swizzle span
-    int bt_log2, bf_log2, bb_log2;      // output tile = 2^bt x 2^bf x 2^bb = 128 positions
-    int tiles_t, tiles_f, tiles_b, tiles_n;
-    int B, F, T;                        // output extents
-    int bn;                             // N tile (output channels per CTA) == wgmma N
-    int nstages;
-    int kind;                           // 0 = tf32, 1 = f16/bf16
-    WsEpi epi;
-};
 
-// persistent / TMA-store variant (ws_gemm_tc2.cu)
+// persistent conv-GEMM on the tensor cores (ws_gemm_tc2.cu)
 struct WsTc2Params {
     CUtensorMap amap[WS_MAX_SRC];
     CUtensorMap amap_lo[WS_MAX_SRC];  // 3xTF32: low parts of the activations
@@ -309,18 +296,17 @@ struct WsTc2Params {
     CUtensorMap imap;     // epilogue input tile (residual, or add2 when has_out2), if has_epin
     WsTcTap taps[WS_MAX_TAPS];
     int ntaps, nk_total;
-    int bk_bytes;
-    int bt_log2, bf_log2, bb_log2;
+    int bk_bytes;                        // 128 / 64 / 32: k-block row bytes == TMA / wgmma swizzle span
+    int bt_log2, bf_log2, bb_log2;       // output tile = 2^bt x 2^bf x 2^bb = 128 positions
     int tiles_t, tiles_f, tiles_b, tiles_n, num_tiles;
-    int B, F, T;
-    int bn, nstages;
-    int kind;
+    int B, F, T;                         // output extents (flattened to 1 x 1 x B*F*T for a dense 1x1 conv)
+    int bn, nstages;                     // N tile (output channels per tile), ring stages
+    int kind;                            // 0 = tf32, 1 = f16/bf16
     int panel_bytes;     // 128 or 64: row bytes of one swizzled staging panel
     int has_out2, has_epin;
     int nsplit;          // 1, or 3 = 3xTF32 error-compensated passes (x_lo*W, x*W_lo, x*W)
     int nout;            // number of output tiles staged per tile (1..4)
     int epi_generic;     // test knob (WS_EPI_GENERIC=1): always run the generic epilogue instantiation
-    int dbg_shift;       // -1 off; else experiment: A tile loaded one row early, MMA reads from row 1 with this base_offset
     int grid, smem_bytes;
     int cl;              // CTAs per cluster: 1, or 2 / 4 (ws_tc3_launch) sharing the weight tile by TMA multicast
     WsEpi epi;
@@ -468,8 +454,6 @@ const char* ws_tc3_launch(const WsTc2Params* p, cudaStream_t s);
 const char* ws_tc2_init(void);
 int ws_tc2_max_smem(void);
 const char* ws_tc2_launch(const WsTc2Params* p, cudaStream_t s);
-const char* ws_tc_init(void);
-const char* ws_tc_launch(const WsTcParams* p, cudaStream_t s);
 const char* ws_simt_launch(const WsSimtParams* p, cudaStream_t s);
 #ifdef __cplusplus
 }

@@ -186,33 +186,30 @@ static int ilog2(int v) {
     return l;
 }
 
-static bool build_tc(const ConvSpec& s, WsTcParams* p) {
-    memset(p, 0, sizeof(*p));
+// Operand side of the tensor-core conv: the k-block size, the taps in k-blocks, the output tile of 128 positions and the
+// activation maps (with their 3xTF32 low twins).  The N tile is chosen by build_tc2.
+static bool tc2_geometry(const ConvSpec& s, WsTc2Params* q) {
     const int es = ws_esize(s.dt);
-    p->kind = s.dt == WS_F32 ? 0 : 1;
-    if (s.Cout % 16 != 0) { set_err("tc conv: Cout must be a multiple of 16"); return false; }
+    q->kind = s.dt == WS_F32 ? 0 : 1;
     if ((int)s.taps.size() > WS_MAX_TAPS) { set_err("tc conv: too many taps"); return false; }
     int minb = 1 << 30;
     for (const WsTap& t : s.taps) minb = std::min(minb, t.nch * es);
-    p->bk_bytes = minb >= 128 ? 128 : (minb >= 64 ? 64 : 32);
     if (minb < 32) { set_err("tc conv: fewer than 32 bytes of channels per tap"); return false; }
-    const int bk_elems = p->bk_bytes / es;
-    p->ntaps = (int)s.taps.size();
-    p->nk_total = 0;
-    for (int i = 0; i < p->ntaps; ++i) {
+    q->bk_bytes = minb >= 128 ? 128 : (minb >= 64 ? 64 : 32);   // k-block row bytes == TMA / wgmma swizzle span
+    const int bk_elems = q->bk_bytes / es;
+    q->ntaps = (int)s.taps.size();
+    for (int i = 0; i < q->ntaps; ++i) {
         const WsTap& t = s.taps[i];
-        WsTcTap& o = p->taps[i];
-        o.map = t.src; o.c0 = t.c0; o.dt = t.dt; o.df = t.df; o.wk = t.wk;
-        o.nkb = (t.nch + bk_elems - 1) / bk_elems;
         if (t.nch % bk_elems != 0 && t.c0 + t.nch != s.src[t.src].C) {
             set_err("tc conv: ragged k-block needs the tap to end at the source view's last channel");
             return false;
         }
-        p->nk_total += o.nkb;
+        q->taps[i] = WsTcTap{t.src, t.c0, t.dt, t.df, t.wk, (t.nch + bk_elems - 1) / bk_elems};
+        q->nk_total += q->taps[i].nkb;
     }
-    // ---- output tile shape
+    // ---- output tile: 128 positions, flat over (B, F, T) for a dense 1x1 conv, else the 2^bt x 2^bf x 2^bb box that pads least
     int B = s.B, F = s.F, T = s.T;
-    bool flat = s.dense_pointwise;
+    const bool flat = s.dense_pointwise;
     int bt = 128, bf = 1, bb = 1;
     const char* env_bt = getenv("WS_TILE_BT");  // tuning knob: minimum time-extent of a non-flat tile
     const int min_bt = env_bt ? atoi(env_bt) : 1;
@@ -229,20 +226,13 @@ static bool build_tc(const ConvSpec& s, WsTcParams* p) {
                 if (best < 0 || cost < best || (cost == best && t > bt)) { best = cost; bt = t; bf = f; bb = b; }
             }
     }
-    p->bt_log2 = ilog2(bt); p->bf_log2 = ilog2(bf); p->bb_log2 = ilog2(bb);
-    p->tiles_t = (T + bt - 1) / bt; p->tiles_f = (F + bf - 1) / bf; p->tiles_b = (B + bb - 1) / bb;
-    p->B = B; p->F = F; p->T = T;
-    p->bn = s.Cout % 128 == 0 ? 128 : (s.Cout % 64 == 0 ? 64 : (s.Cout % 32 == 0 ? 32 : 16));
-    p->tiles_n = s.Cout / p->bn;
-    if ((p->bn * p->bk_bytes) % 1024 != 0) { set_err("tc conv: weight tile not a multiple of the 1024-B swizzle atom"); return false; }
-    const int stage_bytes = (128 + p->bn) * p->bk_bytes;
-    int ns = (96 * 1024) / stage_bytes;
-    p->nstages = ns < 2 ? 2 : (ns > WS_TC_MAX_STAGES ? WS_TC_MAX_STAGES : ns);
-    // ---- tensor maps
+    q->bt_log2 = ilog2(bt); q->bf_log2 = ilog2(bf); q->bb_log2 = ilog2(bb);
+    q->tiles_t = (T + bt - 1) / bt; q->tiles_f = (F + bf - 1) / bf; q->tiles_b = (B + bb - 1) / bb;
+    q->B = B; q->F = F; q->T = T;
+    // ---- activation maps, one per source view (unused slots repeat the first)
     for (int i = 0; i < s.nsrc; ++i) {
         const WsSrc& v = s.src[i];
         cuuint64_t dims[4], str[3];
-        cuuint32_t box[4];
         if (flat) {
             dims[0] = (cuuint64_t)v.C; dims[1] = (cuuint64_t)T; dims[2] = 1; dims[3] = 1;
             str[0] = (cuuint64_t)v.sT * es; str[1] = (cuuint64_t)T * v.sT * es; str[2] = str[1];
@@ -250,37 +240,26 @@ static bool build_tc(const ConvSpec& s, WsTcParams* p) {
             dims[0] = (cuuint64_t)v.C; dims[1] = (cuuint64_t)v.T; dims[2] = (cuuint64_t)v.F; dims[3] = (cuuint64_t)v.B;
             str[0] = (cuuint64_t)v.sT * es; str[1] = (cuuint64_t)v.sF * es; str[2] = (cuuint64_t)v.sB * es;
         }
-        box[0] = (cuuint32_t)bk_elems; box[1] = (cuuint32_t)bt; box[2] = (cuuint32_t)bf; box[3] = (cuuint32_t)bb;
-        if (!encode_map(&p->amap[i], s.dt, v.ptr, 4, dims, str, box, p->bk_bytes)) return false;
+        cuuint32_t box[4] = {(cuuint32_t)bk_elems, (cuuint32_t)bt, (cuuint32_t)bf, (cuuint32_t)bb};
+        if (!encode_map(&q->amap[i], s.dt, v.ptr, 4, dims, str, box, q->bk_bytes)) return false;
+        q->amap_lo[i] = q->amap[i];
+        if (s.split && !encode_map(&q->amap_lo[i], s.dt, v.ptr_lo, 4, dims, str, box, q->bk_bytes)) return false;
     }
-    for (int i = s.nsrc; i < WS_MAX_SRC; ++i) p->amap[i] = p->amap[0];
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)s.Ktot, (cuuint64_t)s.Cout};
-        cuuint64_t str[1] = {(cuuint64_t)s.Ktot * es};
-        cuuint32_t box[2] = {(cuuint32_t)bk_elems, (cuuint32_t)p->bn};
-        if (!encode_map(&p->wmap, s.dt, s.W, 2, dims, str, box, p->bk_bytes)) return false;
-    }
-    p->epi = s.epi;
+    for (int i = s.nsrc; i < WS_MAX_SRC; ++i) { q->amap[i] = q->amap[0]; q->amap_lo[i] = q->amap_lo[0]; }
     return true;
 }
 
-
-// ---- v2 (persistent, TMA-store epilogue).  Returns false *without* error if the spec needs the v1 kernel.
+// ---- the persistent tensor-core kernel (ws_gemm_tc2.cu).  cl: CTAs per cluster sharing the weight tile (1, or 2 / 4:
+// ws_tc3_launch).  Returns false with *unsupported set and no error when no N tile suits a cluster of cl >= 2 CTAs (the
+// caller then builds the layer with cl = 1); every other refusal is an error that names the reason.
 static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int cl = 1) {
-    const bool pair = cl >= 2;   // cl: CTAs per cluster sharing the weight tile (1, or 2 / 4: ws_tc3_launch)
+    const bool pair = cl >= 2;
     *unsupported = false;
     const WsEpi& e = s.epi;
-    if ((e.res != nullptr && e.out2 != nullptr) || s.Cout % 32 != 0) { *unsupported = true; return false; }
-    WsTcParams v1;
-    if (!build_tc(s, &v1)) return false;
+    if (s.Cout % 32 != 0) { set_err("tc conv: Cout must be a multiple of 32 (the narrowest N tile)"); return false; }
+    if (e.res != nullptr && e.out2 != nullptr) { set_err("tc conv: a residual and a second output (out2) cannot be combined"); return false; }
     memset(q, 0, sizeof(*q));
     const int es = ws_esize(s.dt);
-    for (int i = 0; i < WS_MAX_SRC; ++i) q->amap[i] = v1.amap[i];
-    memcpy(q->taps, v1.taps, sizeof(v1.taps));
-    q->ntaps = v1.ntaps; q->nk_total = v1.nk_total; q->bk_bytes = v1.bk_bytes;
-    q->bt_log2 = v1.bt_log2; q->bf_log2 = v1.bf_log2; q->bb_log2 = v1.bb_log2;
-    q->tiles_t = v1.tiles_t; q->tiles_f = v1.tiles_f; q->tiles_b = v1.tiles_b;
-    q->B = v1.B; q->F = v1.F; q->T = v1.T; q->kind = v1.kind;
     q->has_out2 = e.out2 != nullptr;
     q->has_epin = (e.res != nullptr) || (e.out2 != nullptr);
     q->nsplit = s.split ? 3 : 1;
@@ -291,6 +270,7 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
         for (int i = 0; i < s.nsrc; ++i)
             if (s.src[i].ptr_lo == nullptr) { set_err("tc conv: 3xTF32 source without a lo twin"); return false; }
     }
+    if (!tc2_geometry(s, q)) return false;
     q->nout = (s.split ? 2 : 1) * (q->has_out2 ? 2 : 1);
     const int nstage_bufs = q->nout + (q->has_epin ? 1 : 0);
     const int budget = ws_tc2_max_smem() - 1024;
@@ -333,28 +313,24 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
             const int n = (budget - staging) / stage_bytes;
             if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > max_st ? max_st : n; break; }
         }
-    if (bn == 0) { *unsupported = true; return false; }
+    if (bn == 0) {
+        if (pair) *unsupported = true;
+        else set_err("tc conv: no N tile fits in shared memory beside the epilogue staging");
+        return false;
+    }
     q->bn = bn; q->nstages = nst;
     q->tiles_n = s.Cout / bn;
     q->num_tiles = q->tiles_n * ((mtiles + cl - 1) / cl);
     q->panel_bytes = bn * es >= 128 ? 128 : bn * es;
     const int panel_cols = q->panel_bytes / es;
     const int bk_elems = q->bk_bytes / es;
-    {   // weights map with the v2 N tile
+    {   // weights map with the chosen N tile
         cuuint64_t dims[2] = {(cuuint64_t)s.Ktot, (cuuint64_t)s.Cout};
         cuuint64_t str[1] = {(cuuint64_t)s.Ktot * es};
         cuuint32_t box[2] = {(cuuint32_t)bk_elems, (cuuint32_t)(bn / cl)};   // the rows ONE CTA loads per k-block
         if (!encode_map(&q->wmap, s.dt, s.W, 2, dims, str, box, q->bk_bytes)) return false;
         q->wmap_lo = q->wmap;
         if (s.split && !encode_map(&q->wmap_lo, s.dt, s.W_lo, 2, dims, str, box, q->bk_bytes)) return false;
-    }
-    for (int i = 0; i < WS_MAX_SRC; ++i) q->amap_lo[i] = q->amap[i];
-    if (s.split) {   // lo twins of the activation maps: same geometry, different base pointer
-        ConvSpec lo = s;
-        for (int i = 0; i < lo.nsrc; ++i) lo.src[i].ptr = lo.src[i].ptr_lo;
-        WsTcParams v1lo;
-        if (!build_tc(lo, &v1lo)) return false;
-        for (int i = 0; i < WS_MAX_SRC; ++i) q->amap_lo[i] = v1lo.amap[i];
     }
     // output / epilogue-input maps: same tile geometry as the A maps over the output positions
     const bool flat = s.dense_pointwise;
@@ -387,8 +363,6 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     if (pair) q->grid = cl * (q->num_tiles < ncl ? q->num_tiles : ncl);
     else q->grid = q->num_tiles < g_num_sms ? q->num_tiles : g_num_sms;
     q->smem_bytes = nst * (128 + bn) * q->bk_bytes + staging_bytes(bn) + 1024;
-    const char* env_sh = getenv("WS_TC2_SHIFT_TEST");
-    q->dbg_shift = env_sh ? atoi(env_sh) : -1;
     return true;
 }
 
@@ -436,25 +410,16 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
     if (use_tc >= 2) {
         auto q = std::make_shared<WsTc2Params>();
         bool unsupported = false;
-        if (build_tc2(spec, q.get(), &unsupported)) {
-            out->run = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
-            label_conv(out, "conv_tc2", spec);
-            return true;
-        }
-        if (!unsupported) return false;
+        if (!build_tc2(spec, q.get(), &unsupported)) return false;
+        out->run = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
+        label_conv(out, "conv_tc2", spec);
+        return true;
     }
     if (spec.epi.colsum != nullptr) { set_err("conv colsum: only the persistent tensor-core kernels (use_tc >= 2) produce column sums"); return false; }
-    if (use_tc) {
-        auto p = std::make_shared<WsTcParams>();
-        if (!build_tc(spec, p.get())) return false;
-        out->run = [p](cudaStream_t s) { return ws_tc_launch(p.get(), s); };
-        label_conv(out, "conv_tc1", spec);
-    } else {
-        auto p = std::make_shared<WsSimtParams>();
-        if (!build_simt(spec, p.get())) return false;
-        out->run = [p](cudaStream_t s) { return ws_simt_launch(p.get(), s); };
-        label_conv(out, "conv_simt", spec);
-    }
+    auto p = std::make_shared<WsSimtParams>();
+    if (!build_simt(spec, p.get())) return false;
+    out->run = [p](cudaStream_t s) { return ws_simt_launch(p.get(), s); };
+    label_conv(out, "conv_simt", spec);
     return true;
 }
 
@@ -834,6 +799,10 @@ bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int 
 extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
     using namespace ws;
     if (d == nullptr) { set_err("ws_conv: null descriptor"); return 1; }
+    if (d->use_tc < 0 || d->use_tc == 1) {
+        set_err("ws_conv: use_tc must be 0 (FFMA) or 2..4 (tensor cores); 1, the one-tile-per-CTA tensor-core kernel, was removed");
+        return 1;
+    }
     View x;
     x.p = const_cast<void*>(d->x); x.plo = const_cast<void*>(d->x_lo); x.B = d->B; x.F = d->F; x.T = d->T; x.C = d->Cin; x.ld = d->x_ld; x.dt = d->dtype;
     ConvSpec s;
@@ -854,7 +823,7 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
     s.epi.res = d->res; s.epi.res_ld = d->res_ld; s.epi.act2 = d->act2;
     s.epi.colsum = d->colsum; s.epi.colsum_T = d->colsum ? To : 0;
     PlanOp op;
-    if (d->use_tc) { WS_CKS(ws_tc_init()); WS_CKS(ws_tc2_init()); WS_CKS(ws_tc3_init()); WS_CKS(ws_c3_init()); WS_CKS(ws_astp_init()); }
+    if (d->use_tc) { WS_CKS(ws_tc2_init()); WS_CKS(ws_tc3_init()); WS_CKS(ws_c3_init()); WS_CKS(ws_astp_init()); }
     bool done = false;
     if (d->use_tc >= 4 && d->kf == 3 && d->kt == 3 && d->dil_f == 1 && d->dil_t == 1 && d->pad_f == 1 && d->pad_t == 1 &&
         d->stride_f >= 1 && d->stride_f <= 2 && d->stride_t >= 1 && d->stride_t <= 2 && d->scale == nullptr && d->x_lo == nullptr && d->colsum == nullptr &&

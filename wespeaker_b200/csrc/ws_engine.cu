@@ -66,7 +66,7 @@ struct ws_engine {
     std::string model, prec;
     int feat_dim = 80, embed_dim = 0, device = 0;
     int act_dt = WS_F32;
-    int use_tc = 0;  // 0 FFMA, 1 tensor-core v1, 2 tensor-core v2 (persistent), 3 v2 + weight-sharing clusters on large layers (default)
+    int use_tc = 0;  // 0 FFMA, 2 persistent tensor-core kernel, 3 the same + weight-sharing clusters on large layers (default)
     bool split = false;  // 3xTF32: fp32 activations/weights carry lo twins, GEMMs run 3 error-compensated passes
     std::map<const void*, const void*> wlo;  // packed weight -> its lo twin
     std::map<std::string, long long> opts;
@@ -1855,7 +1855,6 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
     WS_CK(cudaSetDevice(device));
     std::unique_ptr<ws_engine> e(new ws_engine());
     if (configure_engine(e.get(), model_name, precision, feat_dim, embed_dim, device)) return 1;
-    WS_CKS(ws_tc_init());
     WS_CKS(ws_tc2_init());
     WS_CKS(ws_res2_init());
     WS_CKS(ws_astp_init());
@@ -1888,7 +1887,14 @@ int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
     if (!e || !key) { set_err("ws_engine_set_option: null argument"); return 1; }
     const std::string k = key;
     if (k == "force_simt") { if (value) e->use_tc = 0; }
-    else if (k == "tc_version") { if (e->use_tc) e->use_tc = value >= 3 ? 3 : (value >= 2 || e->split ? 2 : 1); }
+    else if (k == "tc_version") {
+        if (value != 2 && value != 3) {
+            set_err("tc_version must be 2 (persistent tensor-core kernel) or 3 (+ weight-sharing clusters); 1, the one-tile-per-CTA "
+                    "kernel, was removed");
+            return 1;
+        }
+        if (e->use_tc) e->use_tc = (int)value;
+    }
     else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "plan_lanes" && k != "conv3x3_strided" && k != "astp_fused") { set_err("unknown option " + k); return 1; }
     e->opts[k] = value;
     e->plans.clear();

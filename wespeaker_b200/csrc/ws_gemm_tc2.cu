@@ -1,7 +1,9 @@
-// Persistent warp-specialised conv/GEMM on the Hopper tensor cores (wgmma + TMA, sm_90a), version 2.
+// Persistent warp-specialised conv/GEMM on the Hopper tensor cores (wgmma + TMA, sm_90a).
 //
-// Same operator as ws_gemm_tc.cu (taps over rank-4 TMA maps, 128 positions x bn channels per tile, K-major swizzled
-// operands) with:
+// A conv is an implicit GEMM over output positions: each tap (kernel offset) is a rank-4 TMA map over the channels-last
+// activations, shifted by the tap's time / frequency offset, whose out-of-bounds zero fill is the conv's zero padding.  A
+// tile is 128 output positions x bn output channels; the k loop walks the taps in k-blocks of 128 / 64 / 32 bytes, with A
+// (activations) and B (weights) K-major and swizzled in shared memory as TMA writes them.  On top of that:
 //   * persistent CTAs (one per SM) walking a static tile schedule; the TMA producer runs ahead into the next tile's
 //     operands while the consumers finish the current tile's epilogue;
 //   * bn up to 128: each of the two consumer warpgroups keeps a 64 x bn fp32 accumulator in registers;
@@ -21,6 +23,9 @@
 //
 // Warp roles (384 threads): w0 TMA producer, w1..w3 idle (BN = 256: parameter, store and column-sum warps),
 // w4..w11 two consumer warpgroups (MMA + epilogue).
+//
+// Replaces the library-dispatched cuDNN conv + elementwise launches of wespeaker/models/ecapa_tdnn.py:85-106,
+// resnet.py:35-69, campplus.py:55-83,138-170.
 #include "ws_tc_common.cuh"
 
 namespace {
@@ -144,7 +149,7 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
                             mbar_expect_tx(bar_full + 8 * s, (uint32_t)stage_bytes);
                             const uint32_t sa = ring + (uint32_t)(s * stage_bytes);
                             tma_load_4d(sa, ps == 0 ? &p.amap_lo[tap.map] : &p.amap[tap.map], bar_full + 8 * s,
-                                        tap.c0 + kb * bk_elems, t0 + tap.dt - (p.dbg_shift >= 0 ? 1 : 0), f0 + tap.df, b0);
+                                        tap.c0 + kb * bk_elems, t0 + tap.dt, f0 + tap.df, b0);
                             if constexpr (CL == 1)
                                 tma_load_2d(sa + (uint32_t)a_bytes, ps == 1 ? &p.wmap_lo : &p.wmap, bar_full + 8 * s,
                                             tap.wk + kb * bk_elems, n0);
@@ -280,9 +285,7 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
             for (int kit = 0; kit < nkit; ++kit) {
                 mbar_wait(bar_full + 8 * s, ph);
                 const uint32_t sa = ring + (uint32_t)(s * stage_bytes) + (uint32_t)(wg * 64 * p.bk_bytes);
-                uint64_t adesc = ws_wg::desc(sa, p.bk_bytes);
-                if (p.dbg_shift >= 0)  // row-shifted operand read: start one row in, base_offset field [49,52)
-                    adesc = ws_wg::desc(sa + (uint32_t)p.bk_bytes, p.bk_bytes) | ((uint64_t)(p.dbg_shift & 7) << 49);
+                const uint64_t adesc = ws_wg::desc(sa, p.bk_bytes);
                 const uint64_t bdesc = ws_wg::desc(ring + (uint32_t)(s * stage_bytes + a_bytes), p.bk_bytes);
                 ws_wg::fence();
                 if constexpr (BN == 256) {

@@ -107,7 +107,7 @@ inline std::string tview(const char* n, const View& v) {
 
 // Build a launch closure for `spec`; use_tc selects a tensor-core kernel (needs dt-aligned shapes) else FFMA.
 // Returns false and sets the error string if the spec cannot be mapped.
-bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out);  // 0 FFMA, 1 tensor-core v1, 2 persistent v2 (falls back to v1), 3 v2 with clusters on large layers
+bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out);  // 0 FFMA, 2 persistent tensor-core kernel, 3 the same with clusters on large layers
 
 void fill_epi_out(WsEpi& e, const View& out);
 

@@ -6,7 +6,8 @@
 //   * the conv input s_i = sp_{i-1} + x_i lives in shared memory as a K-major 128B-swizzled operand buffer with zero rows
 //     around it; the three dilated taps are three wgmma operand reads of the SAME buffer at row offsets -d, 0, +d
 //     (the descriptor start address is shifted by whole 128-B rows; the swizzle is a function of the absolute smem
-//     address, tools/shift_probe.py), so there is no im2col, no halo exchange, and the intermediate never goes to HBM;
+//     address: a wrong row-shifted read fails the GPU parity test test_res2_fused_chain_matches_unfused), so there is no
+//     im2col, no halo exchange, and the intermediate never goes to HBM;
 //   * weights stream through a TMA ring (they are L2-resident, shared by all CTAs); each of the two consumer warpgroups
 //     keeps the accumulator of its 64 rows of every 128-row M tile in registers;
 //   * the epilogue (bias, ReLU, BN affine) writes sp_i to the output buffer through a swizzled staging tile + TMA store
@@ -16,56 +17,10 @@
 //     64-row TMA boxes per channel panel); rows before t = 0 and behind the utterance's end are forced to zero in the operand
 //     buffer - they are the convs' zero padding.
 // Warp roles (384 threads): w0 TMA producer, w1..w3 idle, w4..w11 two consumer warpgroups (MMAs + epilogue).
-#include "ws_common.cuh"
-#include "ws_wgmma.cuh"
+#include "ws_tc_common.cuh"
 
 namespace {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-            "r"(dst),
-        "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::
-            "r"(dst),
-        "l"(map), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map),
-                 "r"(src), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+using namespace ws_tcdev;
 
 constexpr int kPadRows = 8;      // zero rows before t=0 (>= max dilation, multiple of 8 keeps the swizzle phase = t & 7)
 constexpr int kSRows = 256 + 16; // operand buffer rows per K panel

@@ -39,8 +39,6 @@ __device__ __forceinline__ void fence_regs(float* d) {
 }
 
 #define WS_WG_F8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
-#define WS_WG_REGS_N16 "{%0, %1, %2, %3, %4, %5, %6, %7}"
-#define WS_WG_OPS_N16 WS_WG_F8(0)
 #define WS_WG_REGS_N32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
 #define WS_WG_OPS_N32 WS_WG_F8(0), WS_WG_F8(8)
 #define WS_WG_REGS_N64 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
@@ -48,18 +46,6 @@ __device__ __forceinline__ void fence_regs(float* d) {
 #define WS_WG_REGS_N128 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
 #define WS_WG_OPS_N128 WS_WG_F8(0), WS_WG_F8(8), WS_WG_F8(16), WS_WG_F8(24), WS_WG_F8(32), WS_WG_F8(40), WS_WG_F8(48), WS_WG_F8(56)
 
-__device__ __forceinline__ void wg_mma_bf16_n16(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\twgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 " WS_WG_REGS_N16
-                 ", %8, %9, p, 1, 1, 0, 0;\n\t}" : WS_WG_OPS_N16 : "l"(da), "l"(db), "r"(acc));
-}
-__device__ __forceinline__ void wg_mma_f16_n16(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\twgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 " WS_WG_REGS_N16
-                 ", %8, %9, p, 1, 1, 0, 0;\n\t}" : WS_WG_OPS_N16 : "l"(da), "l"(db), "r"(acc));
-}
-__device__ __forceinline__ void wg_mma_tf32_n16(float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\twgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 " WS_WG_REGS_N16
-                 ", %8, %9, p, 1, 1;\n\t}" : WS_WG_OPS_N16 : "l"(da), "l"(db), "r"(acc));
-}
 __device__ __forceinline__ void wg_mma_bf16_n32(float* d, uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\twgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " WS_WG_REGS_N32
                  ", %16, %17, p, 1, 1, 0, 0;\n\t}" : WS_WG_OPS_N32 : "l"(da), "l"(db), "r"(acc));
@@ -101,10 +87,8 @@ __device__ __forceinline__ void wg_mma_tf32_n128(float* d, uint64_t da, uint64_t
 // new accumulation.  dt is warp-uniform.
 template <int N>
 __device__ __forceinline__ void mma(int dt, float* d, uint64_t da, uint64_t db, uint32_t acc) {
-    static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma N");
-    if constexpr (N == 16) {
-        if (dt == 1) wg_mma_bf16_n16(d, da, db, acc); else if (dt == 2) wg_mma_f16_n16(d, da, db, acc); else wg_mma_tf32_n16(d, da, db, acc);
-    } else if constexpr (N == 32) {
+    static_assert(N == 32 || N == 64 || N == 128, "wgmma N");
+    if constexpr (N == 32) {
         if (dt == 1) wg_mma_bf16_n32(d, da, db, acc); else if (dt == 2) wg_mma_f16_n32(d, da, db, acc); else wg_mma_tf32_n32(d, da, db, acc);
     } else if constexpr (N == 64) {
         if (dt == 1) wg_mma_bf16_n64(d, da, db, acc); else if (dt == 2) wg_mma_f16_n64(d, da, db, acc); else wg_mma_tf32_n64(d, da, db, acc);
@@ -113,12 +97,11 @@ __device__ __forceinline__ void mma(int dt, float* d, uint64_t da, uint64_t db, 
     }
 }
 
-// the same with N chosen at run time (warp-uniform); d holds at least n / 2 floats
+// the same with N (128, 64 or 32) chosen at run time (warp-uniform); d holds at least n / 2 floats
 __device__ __forceinline__ void mma_n(int n, int dt, float* d, uint64_t da, uint64_t db, uint32_t acc) {
     if (n == 128) mma<128>(dt, d, da, db, acc);
     else if (n == 64) mma<64>(dt, d, da, db, acc);
-    else if (n == 32) mma<32>(dt, d, da, db, acc);
-    else mma<16>(dt, d, da, db, acc);
+    else mma<32>(dt, d, da, db, acc);
 }
 
 // m64n256k16 with the 16-bit operand type fixed at compile time (DT: 1 bf16, 2 fp16): 128 accumulator registers per thread
@@ -150,9 +133,9 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// Row-wise access to an accumulator for epilogues written per output row: the warp's 16 rows x NC columns (NC = 64, 32 or
-// 16 starting at column c0 of the fragment) go through a per-warp shared-memory scratch of 16 x kScrPitch floats, after
-// which lane l owns row (l & 15) and the NC/2 consecutive columns starting at (l >> 4) * NC/2.
+// Row-wise access to an accumulator for epilogues written per output row: the warp's 16 rows x NC = 64 columns starting at
+// column c0 of the fragment go through a per-warp shared-memory scratch of 16 x kScrPitch floats, after which lane l owns
+// row (l & 15) and the 32 consecutive columns starting at (l >> 4) * 32.
 constexpr int kScrPitch = 68;   // 16-byte rows reads are conflict-free per quarter warp (row offsets 4 banks apart)
 constexpr int kScrFloats = 16 * kScrPitch;
 template <int NC>
