@@ -103,9 +103,14 @@ int ws_engine_collect(ws_engine* e, int slot);
 /* tuning aid: per-op device time (ms) of the (B,T) plan, measured with CUDA events in sequence context; returns #ops */
 int ws_engine_profile_ops(ws_engine* e, int B, int T, int iters, float* ms_out, int max_ops);
 const char* ws_engine_plan_op_name(ws_engine* e, int B, int T, int i, double* flops_out);   /* label + FLOPs of op i */
-/* plan-check engines only: write the (B,T) launch plan as data (JSON op descriptions + placeholder allocation table + fp32
- * weight sources) so that a test can re-evaluate the plan's arithmetic on the host (tests/plan_interp.py) */
+/* write the (B,T) launch plan as data (JSON op descriptions + allocation table) so that a test can re-evaluate the plan's
+ * arithmetic on the host (tests/plan_interp.py).  Plan-check engines: placeholder addresses + fp32 weight sources.  Real
+ * engines with the option plan_trace = 1: device addresses, every weight and plan-buffer allocation, no weight sources. */
 int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* path);   /* masked: the length-masked plan of (B,T) */
+/* test aid: run ops [first, last) of the (B,T[,masked]) plan eagerly (no CUDA graph) on `stream`, building the plan if
+ * needed; the caller fills the plan's inputs and orders `stream` against other uses of its buffers.  Refused on a plan-check
+ * engine. */
+int ws_engine_run_ops(ws_engine* e, int B, int T, int masked, int first, int last, void* stream);
 /* number of this library's kernels launched by the most recent forward/extract call */
 long long ws_engine_last_launches(const ws_engine* e);
 void ws_engine_destroy(ws_engine* e);

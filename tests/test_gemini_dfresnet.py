@@ -107,26 +107,9 @@ def test_rejects_other_pooling_and_feat_dims():
     assert m.feat_dim == 64 and len(m.plan_check(1, 100)) > 0
 
 
-def run_dwconv3x3(mem, tr):
-    """ws_launch_dwconv3x3: out = relu(depthwise 3x3(x, w) + shift), zero padding, rows behind an utterance's end read as
-    zeros and written as zeros; w and shift are fp32 (never rounded to the activation dtype)."""
-    es = tr["es"]
-    x = mem.view(tr["x"], es)
-    B, F_, T, C = x.shape
-    valid = (np.arange(T)[None, :] < plan_interp._lens(mem, tr, B, T)[:, None])[:, None, :, None]
-    x = x * valid
-    w = mem.vec(tr["w"], C * 9).reshape(C, 3, 3)
-    acc = np.zeros(x.shape)
-    for jf in range(3):
-        for jt in range(3):
-            acc += plan_interp.shifted(x, jf - 1, jt - 1, F_, T) * w[:, jf, jt]
-    out = np.maximum(acc + mem.vec(tr["shift"], C), 0.0) * valid
-    mem.view(tr["out"], es, write=True)[...] = plan_interp.rnd(out, es)
-
-
 @pytest.fixture
-def interp(monkeypatch):
-    monkeypatch.setitem(plan_interp.EXTRA, "dwconv3x3", run_dwconv3x3)
+def interp():
+    """the depthwise 3x3 contract lives in plan_interp"""
     return plan_interp
 
 

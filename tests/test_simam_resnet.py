@@ -118,67 +118,9 @@ def test_plan_check_in_planes_32_and_rejects_others():
         from_synthetic("SimAM_ResNet34_ASP", precision="fp16", in_planes=16).plan_check(1, 120)
 
 
-def _astp_eps(x, logits, eps):
-    a = np.exp(logits - logits.max(axis=1, keepdims=True))
-    a /= a.sum(axis=1, keepdims=True)
-    mean = (a * x).sum(axis=1)
-    var = (a * x * x).sum(axis=1) - mean * mean
-    return np.concatenate([mean, np.sqrt(np.maximum(var, eps))], axis=1)
-
-
-def run_astp_fused(mem, tr):
-    """make_astp_op with its variance floor (ws_host.h): logits = h @ W2^T, linear2's bias cancels in the softmax."""
-    es = tr["es"]
-    x, h = mem.view(tr["x"], es)[:, 0], mem.view(tr["h"], es)[:, 0]
-    B, T, C = x.shape
-    W2 = plan_interp.rnd(mem.vec(tr["W2"], C * 128).reshape(C, 128), es)
-    lens = plan_interp._lens(mem, tr, B, T)
-    st = mem.strided(tr["stats"], 4, (B, 2 * C), (2 * C, 1), write=True)
-    for b in range(B):
-        st[b] = _astp_eps(x[b:b + 1, :lens[b]], h[b:b + 1, :lens[b]] @ W2.T, tr.get("eps", 1e-7))[0]
-
-
-def run_astp_stats(mem, tr):
-    es = tr["es"]
-    x, lg = mem.view(tr["x"], es)[:, 0], mem.view(tr["logits"], es)[:, 0]
-    B, T, C = x.shape
-    lens = plan_interp._lens(mem, tr, B, T)
-    st = mem.strided(tr["stats"], 4, (B, 2 * C), (2 * C, 1), write=True)
-    for b in range(B):
-        st[b] = _astp_eps(x[b:b + 1, :lens[b]], lg[b:b + 1, :lens[b]], tr.get("eps", 1e-7))[0]
-
-
-def run_simam_stats(mem, tr):
-    """ws_launch_simam_stats: stats [B][2][C] = mean, sum of centred squares / (F*T_b - 1) over each utterance's frames."""
-    x = mem.view(tr["x"], tr["es"])
-    B, F_, T, C = x.shape
-    lens = plan_interp._lens(mem, tr, B, T)
-    st = mem.strided(tr["stats"], 4, (B, 2, C), (2 * C, C, 1), write=True)
-    for b in range(B):
-        xb = x[b, :, :lens[b]]
-        mu = xb.mean(axis=(0, 1))
-        st[b, 0] = mu
-        st[b, 1] = ((xb - mu) ** 2).sum(axis=(0, 1)) / (F_ * lens[b] - 1)
-
-
-def run_simam_apply(mem, tr):
-    """ws_launch_simam_apply: out = relu(y * sigmoid((y - mean)^2 / (4 (var + lambda)) + 0.5) + res) at out's own strides,
-    rows behind an utterance's end written as zeros."""
-    es = tr["es"]
-    y, res = mem.view(tr["y"], es), mem.view(tr["res"], es)
-    B, F_, T, C = y.shape
-    st = mem.strided(tr["stats"], 4, (B, 2, C), (2 * C, C, 1))
-    mu, var = st[:, 0][:, None, None, :], st[:, 1][:, None, None, :]
-    o = np.maximum(y / (1.0 + np.exp(-((y - mu) ** 2 / (4.0 * (var + tr["lambda"])) + 0.5))) + res, 0.0)
-    o = o * (np.arange(T)[None, :] < plan_interp._lens(mem, tr, B, T)[:, None])[:, None, :, None]
-    mem.strided(tr["out"], es, (B, F_, T, C), (tr["out_sb"], tr["out_sf"], tr["out_st"], 1), write=True)[...] = plan_interp.rnd(o, es)
-
-
 @pytest.fixture
-def interp(monkeypatch):
-    for kind, fn in (("simam_stats", run_simam_stats), ("simam_apply", run_simam_apply), ("astp_fused", run_astp_fused),
-                     ("astp_stats", run_astp_stats)):
-        monkeypatch.setitem(plan_interp.EXTRA, kind, fn)
+def interp():
+    """the SimAM, variance-floor ASTP and every other contract live in plan_interp"""
     return plan_interp
 
 

@@ -11,10 +11,13 @@ the plan builders leaves the plans alone:
 The trace's placeholder addresses depend on what was allocated before, so each one is written in canonical form: an
 activation address becomes "A<k>+<offset>" with allocations numbered in order of first reference (header, then ops), and a
 weight address becomes "W<sha256 of its fp32 source>+<offset>".  --out DIR also writes each case's canonical plan to
-DIR/<case>.json, for diffing the cases whose digests differ.
+DIR/<case>.json, for diffing the cases whose digests differ.  --strip-added drops the optional buffer fields (the 3xTF32
+lo twins plo, p_lo, W_lo, out_lo, out2_lo, the linear split-K workspace wsp and the SimAM partial sums) before digesting, for comparing with builds
+whose traces did not name them.
 """
 import argparse
 import bisect
+import functools
 import hashlib
 import json
 import multiprocessing
@@ -30,6 +33,7 @@ from wespeaker_b200.models import SUPPORTED_MODELS, from_synthetic  # noqa: E402
 
 PRECISIONS = ("fp32", "tf32", "tf32x3", "bf16", "fp16")
 PLACEHOLDER = 0x7000000000   # plan_check_alloc hands out addresses from here up
+ADDED_FIELDS = ("plo", "p_lo", "W_lo", "out_lo", "out2_lo", "wsp", "partial")
 
 
 def cases():
@@ -70,8 +74,18 @@ def case_id(c):
     return "_".join([name, prec, f"B{B}", f"T{T}"] + (["masked"] if masked else []) + tags)
 
 
-def canonical(path):
+def _strip_added(x):
+    if isinstance(x, dict):
+        return {k: _strip_added(v) for k, v in x.items() if k not in ADDED_FIELDS}
+    if isinstance(x, list):
+        return [_strip_added(v) for v in x]
+    return x
+
+
+def canonical(path, strip_added=False):
     meta, blob = load_trace(path)
+    if strip_added:
+        meta = {**meta, "ops": _strip_added(meta["ops"])}
     allocs = sorted((a, n) for a, n in meta["allocs"])
     starts = [a for a, _ in allocs]
     weights = {a: hashlib.sha256(blob[o:o + n].tobytes()).hexdigest() for a, o, n in meta["blobs"]}
@@ -102,7 +116,7 @@ def canonical(path):
     return json.dumps({"header": header, "ops": ops}, indent=0, sort_keys=True)
 
 
-def digest(c):
+def digest(c, strip_added=False):
     name, prec, B, T, masked, args, opts = c
     m = from_synthetic(name, 0, precision=prec, **args)
     for k, v in opts.items():
@@ -110,7 +124,7 @@ def digest(c):
     with tempfile.TemporaryDirectory() as d:
         path = os.path.join(d, "plan.wspt")
         m.plan_trace(path, B, T, masked)
-        text = canonical(path)
+        text = canonical(path, strip_added)
     return case_id(c), hashlib.sha256(text.encode()).hexdigest(), text.count('"label"'), text
 
 
@@ -118,12 +132,13 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", help="also write each case's canonical plan to OUT/<case>.json")
     ap.add_argument("--jobs", type=int, default=os.cpu_count())
+    ap.add_argument("--strip-added", action="store_true", help="digest without the optional buffer fields")
     args = ap.parse_args()
     if args.out:
         os.makedirs(args.out, exist_ok=True)
     cs = cases()
     with multiprocessing.get_context("spawn").Pool(args.jobs) as pool:
-        for cid, h, nops, text in pool.imap(digest, cs):
+        for cid, h, nops, text in pool.imap(functools.partial(digest, strip_added=args.strip_added), cs):
             print(f"{cid} {nops} ops {h}", flush=True)
             if args.out:
                 with open(os.path.join(args.out, cid + ".json"), "w") as f:

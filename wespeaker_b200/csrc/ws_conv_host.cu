@@ -21,11 +21,15 @@ static thread_local bool g_plan_check = false;
 bool plan_check_mode() { return g_plan_check; }
 PlanCheckScope::PlanCheckScope(bool on) : prev(g_plan_check) { g_plan_check = on; }
 PlanCheckScope::~PlanCheckScope() { g_plan_check = prev; }
+static thread_local bool g_plan_trace = false;
+bool plan_trace_mode() { return g_plan_trace; }
+PlanTraceScope::PlanTraceScope(bool on) : prev(g_plan_trace) { g_plan_trace = on; }
+PlanTraceScope::~PlanTraceScope() { g_plan_trace = prev; }
 static std::string conv_trace(const ConvSpec& s) {
     std::string j = "{\"kind\":\"conv\"," + ti("es", ws_esize(s.dt)) + ",\"src\":[";
     for (int i = 0; i < s.nsrc; ++i) {
         const WsSrc& v = s.src[i];
-        j += std::string(i ? "," : "") + "{" + tp("p", v.ptr) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," +
+        j += std::string(i ? "," : "") + "{" + tp("p", v.ptr) + (s.split ? tplo("p_lo", v.ptr_lo) : std::string()) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," +
              ti("sB", v.sB) + "," + ti("sF", v.sF) + "," + ti("sT", v.sT) + "}";
     }
     j += "],\"taps\":[";
@@ -39,7 +43,7 @@ static std::string conv_trace(const ConvSpec& s) {
          "," + tp("bias", e.bias) + "," + tp("rowbias", e.rowbias) + "," + ti("rowbias_ld", e.rowbias_ld) + "," + ti("act1", e.act1) + "," + tp("scale", e.scale) +
          "," + tp("shift", e.shift) + "," + tp("gate", e.gate) + "," + ti("gate_ld", e.gate_ld) + "," + ti("gate_seg", e.gate_seg) + "," + ti("gate_nseg", e.gate_nseg) + "," + tp("res", e.res) + "," + ti("res_ld", e.res_ld) + "," + ti("act2", e.act2) + "," + tp("out", e.out) +
          "," + ti("out_ld", e.out_ld) + "," + tp("out2", e.out2) + "," + ti("out2_ld", e.out2_ld) + "," + tp("add2", e.add2) + "," + ti("add2_ld", e.add2_ld) +
-         "," + tp("colsum", e.colsum) + "}";
+         "," + tp("colsum", e.colsum) + (s.split ? tplo("W_lo", s.W_lo) + tplo("out_lo", e.out_lo) + tplo("out2_lo", e.out2_lo) : std::string()) + "}";
     return j;
 }
 
@@ -388,7 +392,7 @@ static void label_conv(PlanOp* op, const char* kern, const ConvSpec& spec) {
     op->flops = 2.0 * pos * spec.Ktot * spec.Cout;
 }
 bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
-    if (plan_check_mode()) out->trace = conv_trace(spec);
+    if (plan_trace_mode()) out->trace = conv_trace(spec);
     const char* env_mp = getenv("WS_TC3_MIN_POS");
     const long long min_pos = env_mp ? atoll(env_mp) : 132LL * 128;   // one wave of 128-row tiles on an H100
     if (use_tc >= 3 && (long long)spec.B * spec.F * spec.T >= min_pos) {
@@ -460,7 +464,7 @@ bool make_res2_op(const View& x, const View& out, const void* W7, const float* b
     const long long units = (long long)x.B * q->ntile;
     q->grid = (int)(units < ws_num_sms() ? units : ws_num_sms());
     op->run = [q](cudaStream_t s) { return ws_res2_launch(q.get(), s); };
-    if (plan_check_mode())
+    if (plan_trace_mode())
         op->trace = "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W7", W7) + "," + tp("bias", bias) +
                     "," + tp("scale", scale) + "," + tp("shift", shift) + "," + ti("w8", w8) + "," + ti("dil", dil) + "," + tp("lens", lens) + "}";
     char buf[160];
@@ -541,7 +545,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
         return true;
     }
     op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
-    if (plan_check_mode())
+    if (plan_trace_mode())
         op->trace = "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) +
                     "," + tp("lens", lens) + "," + tf("eps", var_floor) + "}";
     char buf[160];
@@ -684,7 +688,7 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
              q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
     op->label = buf;
     op->flops = 2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout;
-    if (plan_check_mode())
+    if (plan_trace_mode())
         op->trace = "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) +
                     "," + (res ? tview("res", *res) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) +
                     "," + tp("lens", lens) + "}";

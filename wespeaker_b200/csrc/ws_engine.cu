@@ -53,6 +53,8 @@ struct Plan {
     int lane = 0;               // which of the engine's streams runs this plan through the device-pointer entry points
     cudaEvent_t done = nullptr; // recorded after every use: a later use on another stream waits for it
     bool check = false;         // built by a plan-check engine: buffers are placeholder addresses, nothing to release
+    // plan-trace engines (option plan_trace): every buffer this plan allocated, (address, bytes), for ws_engine_plan_trace
+    std::vector<std::pair<unsigned long long, unsigned long long>> trace_allocs;
     ~Plan() {
         if (done) cudaEventDestroy(done);
         if (gexec) cudaGraphExecDestroy(gexec);
@@ -77,6 +79,10 @@ struct ws_engine {
     // ws_engine_plan_trace
     std::vector<std::pair<unsigned long long, unsigned long long>> check_allocs;
     std::map<unsigned long long, std::vector<float>> check_blobs;
+    // real engines: every weight allocation (address, bytes), written by ws_engine_plan_trace under the option plan_trace (the
+    // weights are usually uploaded by ws_engine_finalize, before any option is set; a plan's own buffers are in
+    // Plan::trace_allocs: they go away with the plan)
+    std::vector<std::pair<unsigned long long, unsigned long long>> weight_allocs;
     std::map<std::string, void*> wcache;  // packed device weights by id
     std::map<std::pair<int, int>, std::unique_ptr<Plan>> plans;   // key: (B, 2 * T + masked)
     long long last_launches = 0;
@@ -162,6 +168,8 @@ struct Weights {
             if (ok) set_err("device allocation/copy failed for weight " + id);
             ok = false;
             return nullptr;
+        } else {
+            e.weight_allocs.push_back({(unsigned long long)d, (unsigned long long)bytes});
         }
         e.wcache[id] = d;
         return d;
@@ -260,6 +268,8 @@ struct Builder {
             if (ok) set_err("cudaMalloc failed for an activation buffer");
             ok = false;
             return nullptr;
+        } else if (plan_trace_mode()) {
+            p.trace_allocs.push_back({(unsigned long long)d, (unsigned long long)bytes});
         }
         p.bufs.push_back(d);
         p.bytes += bytes;
@@ -284,9 +294,9 @@ struct Builder {
         return v;
     }
     void push(PlanOp op) { p.ops.push_back(std::move(op)); }
-    // a bandwidth op: launch closure, label, and its plan-trace description (kept in plan-check mode only)
+    // a bandwidth op: launch closure, label, and its plan-trace description (kept in plan-trace mode only)
     void push(Op run, const char* label, std::string trace) {
-        push(PlanOp{std::move(run), label, 0.0, plan_check_mode() ? std::move(trace) : std::string()});
+        push(PlanOp{std::move(run), label, 0.0, plan_trace_mode() ? std::move(trace) : std::string()});
     }
     // length-masked plans: frame counts of stride level k (nullptr in ordinary plans), and "zero the rows behind every
     // utterance's end" for tensors a time-mixing op is about to read (the reference's unpadded forward sees zero padding)
@@ -357,7 +367,8 @@ struct Builder {
             return ws_launch_linear_rows(in, in_ld, in2, in2_ld, rows_per_b, W, bias, out, out_ld, R, I, O, act, wsp,
                                          nsplit, s);
         }, "linear_rows", "{\"kind\":\"linear\"," + tp("in", in) + "," + ti("in_ld", in_ld) + "," + tp("in2", in2) + "," + ti("in2_ld", in2_ld) + "," + ti("rows_per_b", rows_per_b) + "," +
-                     tp("W", W) + "," + tp("bias", bias) + "," + tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("R", R) + "," + ti("I", I) + "," + ti("O", O) + "," + ti("act", act) + "}");
+                     tp("W", W) + "," + tp("bias", bias) + "," + tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("R", R) + "," + ti("I", I) + "," + ti("O", O) + "," + ti("act", act) +
+                     tplo("wsp", wsp) + "}");
     }
     // the fp32 input features -> x0 (B,1,T,feat_dim) in the activation dtype
     void convert_input(const View& x0) {
@@ -367,7 +378,7 @@ struct Builder {
         const int dt = x0.dt;
         const long long n = x0.npos() * x0.C;
         push([=](cudaStream_t s) { return ws_launch_convert(fin, xo, xlo, dt, n, s); }, "convert",
-             "{\"kind\":\"convert\"," + ti("es", ws_esize(dt)) + "," + tp("in", fin) + "," + tp("out", xo) + "," + ti("n", n) + "}");
+             "{\"kind\":\"convert\"," + ti("es", ws_esize(dt)) + "," + tp("in", fin) + "," + tp("out", xo) + "," + ti("n", n) + tplo("out_lo", xlo) + "}");
     }
     // out = relu(x * scale + shift), per channel over x's C channels
     void bnrelu(const View& x, const float* scale, const float* shift, const View& out) {
@@ -1140,7 +1151,7 @@ static bool simam(Builder& b, const View& y, const View& res, const View& out, W
     const int* l = b.lens(lvl);
     const int dt = b.e.act_dt;
     b.push([=](cudaStream_t s) { return ws_launch_simam_stats(yv.p, dt, yv.B, yv.F, yv.T, yv.C, yv.ld, partial, stats, s, l); }, "simam_stats",
-           "{\"kind\":\"simam_stats\"," + ti("es", ws_esize(dt)) + "," + tview("x", yv) + "," + tp("stats", stats) + "," + tp("lens", l) + "}");
+           "{\"kind\":\"simam_stats\"," + ti("es", ws_esize(dt)) + "," + tview("x", yv) + "," + tp("stats", stats) + "," + tp("lens", l) + tplo("partial", partial) + "}");
     b.p.extra_launches += 1;   // partials + merge
     b.push([=](cudaStream_t s) {
         return ws_launch_simam_apply(yv.p, yv.ld, stats, kSimamLambda, rv.p, rs, op_, olo, os, dt, yv.B, yv.F, yv.T, yv.C, s, l);
@@ -1525,7 +1536,7 @@ bool build_campplus(Builder& b) {
                 const float* w2cd = b.w.f32("w2ct:" + p, w2ct);
                 const float* b2cd = b.w.vec(p + ".cam_layer.linear2.bias");
                 okl = cam_layer_fill(&hl[(size_t)j - 1], e.act_dt, W1d, Wld, s1d, h1d, h2d, w1cd, b1cd, w2cd, b2cd, cin, dil[bl]);
-                if (plan_check_mode())
+                if (plan_trace_mode())
                     hl_trace[(size_t)j - 1] = "{" + tp("W1", W1d) + "," + tp("Wl", Wld) + "," + tp("bn1_scale", s1d) + "," + tp("bn1_shift", h1d) +
                                               "," + tp("bias2", h2d) + "," + tp("w1c_t", w1cd) + "," + tp("b1c", b1cd) + "," + tp("w2c_t", w2cd) + "," +
                                               tp("b2c", b2cd) + "," + ti("cin", cin) + "," + ti("dil", dil[bl]) + "}";
@@ -1540,7 +1551,7 @@ bool build_campplus(Builder& b) {
                 PlanOp op;
                 bool unsupported = false;
                 if (make_cam_dense_op(X[bl], ldev, j, j1, &op, &unsupported, b.lens(1))) {
-                    if (plan_check_mode()) {   // semantic description of the fused launch: layers [j, j1) over the concat buffer
+                    if (plan_trace_mode()) {   // semantic description of the fused launch: layers [j, j1) over the concat buffer
                         op.trace = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(e.act_dt)) + "," + tview("X", X[bl]) + "," + tp("lens", b.lens(1)) + "," +
                                    ti("seg_len", 100) + ",\"layers\":[";
                         for (int k = j; k < j1; ++k) op.trace += std::string(k > j ? "," : "") + hl_trace[(size_t)k];
@@ -1636,6 +1647,7 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
     std::unique_ptr<Plan> p(new Plan());
     p->B = B; p->T = T; p->masked = masked; p->check = e->plan_check;
     PlanCheckScope check_scope(e->plan_check);
+    PlanTraceScope trace_scope(e->plan_check || e->opt("plan_trace", 0) != 0);
     Builder b(*e, *p);
     if (masked) {
         p->lens = (int*)b.raw((size_t)4 * B * sizeof(int));
@@ -1895,7 +1907,7 @@ int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
         }
         if (e->use_tc) e->use_tc = (int)value;
     }
-    else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "plan_lanes" && k != "conv3x3_strided" && k != "astp_fused") { set_err("unknown option " + k); return 1; }
+    else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "plan_lanes" && k != "conv3x3_strided" && k != "astp_fused" && k != "plan_trace") { set_err("unknown option " + k); return 1; }
     e->opts[k] = value;
     e->plans.clear();
     return 0;
@@ -2271,22 +2283,34 @@ const char* ws_engine_plan_op_name(ws_engine* e, int B, int T, int i, double* fl
     return p->ops[i].label.c_str();
 }
 
-// Plan-check engines only: write the (B,T) launch plan as data - a JSON description of every op (operands as placeholder
-// addresses, shapes, strides, epilogues), the placeholder allocation table and the fp32 source of every weight - so that a
-// test can re-evaluate the plan's arithmetic on the host (tests/plan_interp.py) and compare it with the oracle.
+// Write the (B,T) launch plan as data - a JSON description of every op (operands as addresses, shapes, strides, epilogues),
+// the allocation table and, on plan-check engines, the fp32 source of every weight - so that a test can re-evaluate the
+// plan's arithmetic on the host (tests/plan_interp.py) and compare it with the oracle.  Plan-check engines write placeholder
+// addresses.  Real engines with the option plan_trace = 1 write device addresses, every weight and plan-buffer allocation
+// and no weight blobs (the weights are on the device, in the dtype the kernels read), so that a test can run the plan op by
+// op (ws_engine_run_ops) and check what each kernel wrote.
 // File layout: "WSPT1\n", uint64 JSON length, JSON, then the weight blobs (fp32) back to back; the JSON's "blobs" table
 // holds [address, float offset into the blob area, float count].
 int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* path) {
     if (!e || !path) { set_err("ws_engine_plan_trace: null argument"); return 1; }
-    if (!e->plan_check || !e->finalized) { set_err("ws_engine_plan_trace: needs a finalized plan-check engine"); return 1; }
+    if (!e->finalized || (!e->plan_check && e->opt("plan_trace", 0) == 0)) {
+        set_err("ws_engine_plan_trace: needs a finalized plan-check engine, or a finalized engine with the option plan_trace = 1");
+        return 1;
+    }
+    if (!e->plan_check && cudaSetDevice(e->device) != cudaSuccess) { set_err("ws_engine_plan_trace: cudaSetDevice failed"); return 1; }
     Plan* p = get_plan(e, B, T, masked != 0);
     if (!p) return 1;
+    std::vector<std::pair<unsigned long long, unsigned long long>> allocs = e->check_allocs;
+    if (!e->plan_check) {
+        allocs = e->weight_allocs;
+        allocs.insert(allocs.end(), p->trace_allocs.begin(), p->trace_allocs.end());
+    }
     std::string j = "{";
     j += ti("B", B) + "," + ti("T", T) + "," + ti("feat_dim", e->feat_dim) + "," + ti("embed_dim", e->embed_dim) + "," +
          ti("act_es", ws_esize(e->act_dt)) + "," + tp("feats_in", p->feats_in) + "," + tp("emb", p->emb) + "," + tp("lens", p->lens) + ",\"model\":\"" + e->model +
          "\",\"precision\":\"" + e->prec + "\",\"allocs\":[";
-    for (size_t i = 0; i < e->check_allocs.size(); ++i)
-        j += std::string(i ? "," : "") + "[" + std::to_string(e->check_allocs[i].first) + "," + std::to_string(e->check_allocs[i].second) + "]";
+    for (size_t i = 0; i < allocs.size(); ++i)
+        j += std::string(i ? "," : "") + "[" + std::to_string(allocs[i].first) + "," + std::to_string(allocs[i].second) + "]";
     j += "],\"blobs\":[";
     unsigned long long off = 0;
     bool first = true;
@@ -2310,6 +2334,23 @@ int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* pat
         okw = okw && (kv.second.empty() || fwrite(kv.second.data(), 4, kv.second.size(), f) == kv.second.size());
     okw = (fclose(f) == 0) && okw;
     if (!okw) { set_err(std::string("ws_engine_plan_trace: write failed: ") + path); return 1; }
+    return 0;
+}
+
+// Test aid: run ops [first, last) of the (B,T[,masked]) plan eagerly (no CUDA graph) on `stream`, building the plan if needed.
+// The caller fills the plan's inputs (ws_engine_plan_trace names feats_in and lens) and orders `stream` after whatever else
+// touches the plan's buffers; nothing is synchronised here.
+int ws_engine_run_ops(ws_engine* e, int B, int T, int masked, int first, int last, void* stream) {
+    if (!e) { set_err("ws_engine_run_ops: null engine"); return 1; }
+    if (const char* nr = not_runnable(e)) { set_err(std::string("ws_engine_run_ops") + nr); return 1; }
+    WS_CK(cudaSetDevice(e->device));
+    Plan* p = get_plan(e, B, T, masked != 0);
+    if (!p) return 1;
+    if (first < 0 || last > (int)p->ops.size() || first > last) { set_err("ws_engine_run_ops: op range outside the plan"); return 1; }
+    for (int i = first; i < last; ++i) {
+        const char* m = p->ops[i].run((cudaStream_t)stream);
+        if (m) { set_err("ws_engine_run_ops: op " + std::to_string(i) + " (" + p->ops[i].label + "): " + m); return 1; }
+    }
     return 0;
 }
 

@@ -41,6 +41,14 @@ struct PlanCheckScope {
     ~PlanCheckScope();
 };
 void* plan_check_alloc(size_t bytes);   // 256-byte aligned placeholder address
+// Plan-trace mode: the builders keep each op's JSON trace (PlanOp::trace).  On in plan-check mode and, on a real engine, with
+// the engine option plan_trace = 1 (ws_engine_plan_trace then writes real device addresses).  Thread-local like the above.
+bool plan_trace_mode();
+struct PlanTraceScope {
+    bool prev;
+    explicit PlanTraceScope(bool on);
+    ~PlanTraceScope();
+};
 
 // channels-last activation view: element (b,f,t,c) at p[((b*F+f)*T+t)*ld + c]
 struct View {
@@ -88,8 +96,9 @@ int add_conv_taps(ConvSpec& spec, const View& x, int kf, int kt, int dil_f, int 
 
 using Op = std::function<const char*(cudaStream_t)>;
 // One op of a launch plan: the launch closure, a label and FLOPs (tuning aid, ws_engine_profile_ops; FLOPs 0 = not GEMM-like)
-// and, in plan-check mode only, a JSON description of the op (operands as placeholder addresses, shapes, strides, epilogue)
-// that ws_engine_plan_trace writes so that a test can re-evaluate the plan's arithmetic on the host against the oracle.
+// and, in plan-trace mode only, a JSON description of the op (operands as addresses, shapes, strides, epilogue) that
+// ws_engine_plan_trace writes so that a test can re-evaluate the plan's arithmetic on the host against the oracle, or check
+// what each kernel of a real engine wrote.
 struct PlanOp {
     Op run;
     std::string label;
@@ -97,12 +106,14 @@ struct PlanOp {
     std::string trace;
 };
 
-// Plan-trace JSON fields: "name":address, "name":integer, "name":float (%.9g), "name":{view}
+// Plan-trace JSON fields: "name":address, "name":integer, "name":float (%.9g), "name":{view}.  Optional buffers - a 3xTF32
+// lo twin, a split-K or partial-sum workspace - are named only where there is one (tplo: ",\"name\":address" or nothing).
 inline std::string tp(const char* n, const void* q) { char b[96]; snprintf(b, sizeof b, "\"%s\":%llu", n, (unsigned long long)q); return b; }
 inline std::string ti(const char* n, long long v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%lld", n, v); return b; }
 inline std::string tf(const char* n, double v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%.9g", n, v); return b; }
+inline std::string tplo(const char* n, const void* q) { return q ? "," + tp(n, q) : std::string(); }
 inline std::string tview(const char* n, const View& v) {
-    return std::string("\"") + n + "\":{" + tp("p", v.p) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
+    return std::string("\"") + n + "\":{" + tp("p", v.p) + tplo("plo", v.plo) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
 }
 
 // Build a launch closure for `spec`; use_tc selects a tensor-core kernel (needs dt-aligned shapes) else FFMA.

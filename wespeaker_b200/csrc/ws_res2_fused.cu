@@ -11,7 +11,8 @@
 //   * weights stream through a TMA ring (they are L2-resident, shared by all CTAs); each of the two consumer warpgroups
 //     keeps the accumulator of its 64 rows of every 128-row M tile in registers;
 //   * the epilogue (bias, ReLU, BN affine) writes sp_i to the output buffer through a swizzled staging tile + TMA store
-//     and writes s_{i+1} = sp_i + x_{i+1} straight back into the operand buffer for the next conv.
+//     and writes s_{i+1} = rnd(sp_i + x_{i+1}) straight back into the operand buffer for the next conv, from the rounded
+//     16-bit sp_i it stores (the unfused chain's contract).
 //   * utterances longer than 256 frames are walked in time tiles of 256 rows that overlap by 2 x 32: the chain's receptive
 //     field is 7 x dilation <= 28 rows per side, so the inner 192 rows of a tile are exact and only those are stored (three
 //     64-row TMA boxes per channel panel); rows before t = 0 and behind the utterance's end are forced to zero in the operand
@@ -177,9 +178,13 @@ __global__ void __launch_bounds__(384, 1) ws_res2_fused_kernel(const __grid_cons
                             const uint32_t oa = sO + (uint32_t)((pn * 256 + t) * 128) + off;
                             uint32_t xs = 0u;
                             if (has_next) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(xs) : "r"(oa));
-                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(oa), "r"(ws_pack2(a0, a1, DT)) : "memory");
+                            const uint32_t sp = ws_pack2(a0, a1, DT);
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(oa), "r"(sp) : "memory");
                             if (has_next && valid) {   // rows >= T stay zero = conv padding
-                                const uint32_t o = ws_pack2(a0 + ws_16_to_f(xs & 0xffffu, DT), a1 + ws_16_to_f(xs >> 16, DT), DT);
+                                // s_{i+1} = rnd(sp_i + x_{i+1}) from the 16-bit sp_i that is stored (as the unfused chain's
+                                // out2 = rnd(rnd(sp_i) + x_{i+1}) does), not from its fp32 value
+                                const uint32_t o = ws_pack2(ws_16_to_f(sp & 0xffffu, DT) + ws_16_to_f(xs & 0xffffu, DT),
+                                                            ws_16_to_f(sp >> 16, DT) + ws_16_to_f(xs >> 16, DT), DT);
                                 asm volatile("st.shared.b32 [%0], %1;" ::"r"(sS + (uint32_t)((pn * kSRows + kPadRows + t) * 128) + off),
                                              "r"(o) : "memory");
                             }

@@ -87,6 +87,7 @@ _PROTOS = {
     "ws_engine_collect": (C.c_int, [c_engine_p, C.c_int]),
     "ws_engine_plan_op_name": (C.c_char_p, [c_engine_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ws_engine_plan_trace": (C.c_int, [c_engine_p, C.c_int, C.c_int, C.c_int, C.c_char_p]),
+    "ws_engine_run_ops": (C.c_int, [c_engine_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ws_engine_profile_ops": (C.c_int, [c_engine_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]),
     "ws_engine_last_launches": (C.c_longlong, [c_engine_p]),
     "ws_engine_destroy": (None, [c_engine_p]),

@@ -168,6 +168,26 @@ class B200SpeakerModel(torch.nn.Module):
         finally:
             L.ws_engine_destroy(h)
 
+    def device_trace(self, path: str, batch: int = 1, frames: int = 200, masked: bool = False, device: int | None = None):
+        """Write the (batch, frames) launch plan of the engine on `device` as data, with device addresses and every weight
+        and plan-buffer allocation (ws_engine_plan_trace on a real engine; needs set_option("plan_trace", 1)).  With
+        run_ops, tests check what each kernel of the plan writes."""
+        L = _lib.load()
+        idx = self._dev_index() if device is None else device
+        h = self._ensure_engine(idx)
+        with torch.cuda.device(idx):
+            _lib.check(L.ws_engine_plan_trace(h, batch, frames, int(masked), path.encode()), "ws_engine_plan_trace")
+
+    def run_ops(self, batch: int, frames: int, masked: bool, first: int, last: int, device: int | None = None):
+        """Run ops [first, last) of the (batch, frames) plan eagerly (no CUDA graph) on the current stream; the caller has
+        filled the plan's inputs (feats_in, and lens in a masked plan, as named by device_trace)."""
+        L = _lib.load()
+        idx = self._dev_index() if device is None else device
+        h = self._ensure_engine(idx)
+        with torch.cuda.device(idx):
+            _lib.check(L.ws_engine_run_ops(h, batch, frames, int(masked), first, last, _lib.cur_stream_ptr(idx)),
+                       "ws_engine_run_ops")
+
     def plan_check(self, batch: int = 1, frames: int = 200):
         """Validate the loaded checkpoint against the engine's plan builder WITHOUT a device (ws_engine_create_plan_check:
         nothing is computed): missing / mis-shaped tensors, kernel envelopes and tensor-map alignment rules raise B200Error.
