@@ -29,6 +29,7 @@ class Memory:
         self.starts = np.array([a for a, _ in self.allocs], dtype=np.uint64)
         self.bufs = {}      # base address -> (float64 array, element size)
         self.writes = []    # (address, element size, shape, element strides) of every region an op's contract writes
+        self.reads = []     # (address, element size, shape, element strides) of every region an op's contract reads
         self.blobs = {a: blob[o:o + n].astype(np.float64) for a, o, n in meta["blobs"]}
 
     def _find(self, addr):
@@ -54,17 +55,27 @@ class Memory:
         """n elements at addr; es is the size the operand is stored in (weights in the activation dtype: 2 in 16-bit plans)"""
         if not addr:
             return None
+        self.reads.append((addr, es, (n,), (1,)))
         arr, off = self.array(addr, es)
         return arr[off:off + n]
+
+    def read(self, addr, es, shape, strides):
+        """declare a region the contract reads without going through strided / view (in-place ops)"""
+        self.reads.append((addr, es, tuple(shape), tuple(strides)))
 
     def strided(self, addr, es, shape, strides, write=False):
         if write:
             self.writes.append((addr, es, tuple(shape), tuple(strides), None, False))
+        else:
+            self.reads.append((addr, es, tuple(shape), tuple(strides)))
+        return self.region(addr, es, shape, strides, write)
+
+    def region(self, addr, es, shape, strides, writeable=True):
+        """array over a region, recorded as neither read nor written"""
         arr, off = self.array(addr, es)
         need = off + sum((s - 1) * st for s, st in zip(shape, strides)) + 1
         assert need <= arr.size, (addr, shape, strides, arr.size)
-        v = np.lib.stride_tricks.as_strided(arr[off:], shape=shape, strides=[st * 8 for st in strides], writeable=write)
-        return v
+        return np.lib.stride_tricks.as_strided(arr[off:], shape=shape, strides=[st * 8 for st in strides], writeable=writeable)
 
     def side(self, addr):
         """declare the rest of addr's allocation as an op's scratch / side output: it may change, its values are not checked
@@ -222,7 +233,7 @@ def run_conv3x3(mem, tr):
         mag += np.abs(mem.view(tr["res"], es))
     acc = {0: acc, 1: np.maximum(acc, 0.0), 2: np.clip(acc, 0.0, 20.0)}[tr["relu"]]
     if tr["lens"]:      # length-masked batch: output rows behind an utterance's end are stored as zeros
-        acc = acc * (np.arange(To)[None, :] < mem.vec(tr["lens"], o["B"])[:, None])[:, None, :, None]
+        acc = np.where((np.arange(To)[None, :] < mem.vec(tr["lens"], o["B"])[:, None])[:, None, :, None], acc, 0.0)
     mem.view(o, es, write=True)[...] = rnd(acc, es)
     return {o["p"]: mag}
 
@@ -234,7 +245,7 @@ def run_stem(mem, tr, meta):
     valid = np.ones((B, T), bool)
     if tr["lens"]:      # frames behind an utterance's end are padding: read as zeros, written as zeros
         valid = np.arange(T)[None, :] < mem.vec(tr["lens"], B)[:, None]
-        feats = feats * valid[:, :, None]
+        feats = np.where(valid[:, :, None], feats, 0.0)
     w9 = mem.vec(tr["w9"], C * 9).reshape(C, 9)
     x = feats.transpose(0, 2, 1)[..., None]                                # (B,F,T,1)
     acc = np.zeros((B, Fd, T, C))
@@ -243,7 +254,7 @@ def run_stem(mem, tr, meta):
         for jt in range(3):
             acc += shifted(x, jf - 1, jt - 1, Fd, T) * w9[:, jf * 3 + jt]
             mag += np.abs(shifted(x, jf - 1, jt - 1, Fd, T) * w9[:, jf * 3 + jt])
-    acc = np.maximum(acc + mem.vec(tr["shift"], C), 0.0) * valid[:, None, :, None]
+    acc = np.where(valid[:, None, :, None], np.maximum(acc + mem.vec(tr["shift"], C), 0.0), 0.0)
     mem.view(o, tr["es"], write=True)[...] = rnd(acc, tr["es"])
     return {o["p"]: 3.0 * mag + np.abs(mem.vec(tr["shift"], C))}
 
@@ -485,9 +496,14 @@ def run_cam_dense(mem, tr):
     """ws_host.h make_cam_dense_op / campplus.py:86-201, per layer: h = relu(W1 relu(bn1(x[:, :cin])) + bias2) (BN2 folded into
     W1), context mask m = sigmoid(W2c relu(W1c (mean_T(h) + segmean(h)) + b1c) + b2c) per 100-frame segment,
     x[:, cin:cin+32] = (k3 dilated conv of h) * m."""
-    es, L = tr["es"], tr["seg_len"]
-    Xall = mem.view(tr["X"], es, write=True)
-    B, _, Tmax, _ = Xall.shape
+    es, L, V = tr["es"], tr["seg_len"], tr["X"]
+    B, Tmax, ld = V["B"], V["T"], V["ld"]
+    Xall = mem.region(V["p"], es, (B, 1, Tmax, V["C"]), (Tmax * ld, Tmax * ld, ld, 1))
+    # in place over the concat buffer: reads the channels in front of its first layer (whole 128-row tiles, so every row),
+    # writes each layer's 32-channel slice
+    mem.read(V["p"], es, (B, Tmax, tr["layers"][0]["cin"]), (Tmax * ld, ld, 1))
+    for ly in tr["layers"]:
+        mem.writes.append((V["p"] + ly["cin"] * es, es, (B, Tmax, 32), (Tmax * ld, ld, 1), None, False))
     lens = _lens(mem, tr, B, Tmax)
     links = getattr(mem, "links", None)     # check layer by layer: each layer reads the slices the kernel stored
     got = links.view(tr["X"], es) if links is not None else None
@@ -517,12 +533,13 @@ def run_cam_dense(mem, tr):
             Xall[b, 0, T:, cin:cin + 32] = got[b, 0, T:, cin:cin + 32] if got is not None else 0.0
             dy = _dil_conv1d(dh + np.sqrt(3 * 128) * np.abs(h), np.abs(Wl), dil)
             err[b, 0, :T, cin:cin + 32] = (dy * m[:, seg_of_t, :])[0] + 2.0 * np.abs(y * m[:, seg_of_t, :])[0]
-    return {tr["X"]["p"]: err}
+    return {V["p"] + ly["cin"] * es: err[:, 0, :, ly["cin"]:ly["cin"] + 32] for ly in tr["layers"]}
 
 
 def run_lens_derive(mem, tr):
     """frames per utterance behind each stride-2 level: level 0 clamped to [1, T], level k + 1 = (level k - 1) // 2 + 1"""
     B, T, levels = tr["B"], tr["T"], tr["levels"]
+    mem.read(tr["lens"], 4, (B,), (1,))
     lens = mem.strided(tr["lens"], 4, (levels, B), (B, 1), write=True)
     lens[0] = np.clip(lens[0], 1, T)
     for k in range(1, levels):
@@ -533,7 +550,11 @@ def run_lens_derive(mem, tr):
 def run_zero_tail(mem, tr):
     x = mem.view(tr["x"], tr["es"], write=True)
     B, F, T, C = x.shape
-    x *= (np.arange(T)[None, :] < mem.vec(tr["lens"], B)[:, None])[:, None, :, None]
+    lens = mem.vec(tr["lens"], B)
+    v = tr["x"]
+    for b in range(B):      # in place: the rows in front of the utterance's end are read (and kept), the rest written
+        mem.read(v["p"] + b * F * T * v["ld"] * tr["es"], tr["es"], (F, int(min(max(lens[b], 0), T)), C), (T * v["ld"], v["ld"], 1))
+    x[...] = np.where((np.arange(T)[None, :] < lens[:, None])[:, None, :, None], x, 0.0)
     return {tr["x"]["p"]: np.zeros(x.shape)}
 
 
@@ -566,7 +587,7 @@ def run_simam_apply(mem, tr):
     mu, var = st[:, 0][:, None, None, :], st[:, 1][:, None, None, :]
     z = (y - mu) ** 2 / (4.0 * (var + tr["lambda"])) + 0.5
     o = np.maximum(y / (1.0 + np.exp(-z)) + res, 0.0)
-    o = o * (np.arange(T)[None, :] < _lens(mem, tr, B, T)[:, None])[:, None, :, None]
+    o = np.where((np.arange(T)[None, :] < _lens(mem, tr, B, T)[:, None])[:, None, :, None], o, 0.0)
     mem.strided(tr["out"], es, (B, F_, T, C), (tr["out_sb"], tr["out_sf"], tr["out_st"], 1), write=True)[...] = rnd(o, es)
     # a few fp32 roundings on each term; the sigmoid's slope (<= 1/4) carries the relative error of its argument z
     return {tr["out"]: 4.0 * (np.abs(y) + np.abs(res)) + np.abs(y) * (z + 2.0)}
@@ -579,7 +600,7 @@ def run_dwconv3x3(mem, tr):
     x = mem.view(tr["x"], es)
     B, F_, T, C = x.shape
     valid = (np.arange(T)[None, :] < _lens(mem, tr, B, T)[:, None])[:, None, :, None]
-    x = x * valid
+    x = np.where(valid, x, 0.0)
     w = mem.vec(tr["w"], C * 9).reshape(C, 3, 3)
     acc = np.zeros(x.shape)
     mag = np.zeros(x.shape)
@@ -587,7 +608,7 @@ def run_dwconv3x3(mem, tr):
         for jt in range(3):
             acc += shifted(x, jf - 1, jt - 1, F_, T) * w[:, jf, jt]
             mag += np.abs(shifted(x, jf - 1, jt - 1, F_, T) * w[:, jf, jt])
-    out = np.maximum(acc + mem.vec(tr["shift"], C), 0.0) * valid
+    out = np.where(valid, np.maximum(acc + mem.vec(tr["shift"], C), 0.0), 0.0)
     mem.view(tr["out"], es, write=True)[...] = rnd(out, es)
     return {tr["out"]["p"]: 3.0 * mag + np.abs(mem.vec(tr["shift"], C))}
 
@@ -751,16 +772,20 @@ def _elements(shape, strides, off):
     return idx
 
 
+def _byte_mask(t, regions):
+    """bool torch tensor over the bytes of allocation tensor t: True on every byte of the regions (element offset, es,
+    shape, strides, ...)"""
+    import torch
+    mask = torch.zeros(t.numel(), dtype=torch.bool, device=t.device)
+    for off, es, shape, strides, *_ in regions:
+        el = torch.from_numpy(_elements(shape, strides, off).reshape(-1)).to(t.device)
+        mask[:t.numel() // es * es].view(-1, es)[el] = True
+    return mask
+
+
 def declared_mask(raw, regions, base):
     """bool torch tensor over the bytes of allocation `base`: True where the op may write"""
-    import torch
-    t = raw[base]
-    mask = torch.zeros(t.numel(), dtype=torch.bool, device=t.device)
-    for off, es, shape, strides, _, _ in regions.get(base, []):
-        el = torch.from_numpy(_elements(shape, strides, off).reshape(-1)).to(t.device)
-        for k in range(es):
-            mask[el * es + k] = True
-    return mask
+    return _byte_mask(raw[base], regions.get(base, []))
 
 
 def perfect_outputs(meta, before, ref):
@@ -793,27 +818,67 @@ C_KIND = {"conv": 2.0, "conv3x3": 2.0, "stem": 2.0, "res2_fused": 2.0, "linear":
           "dwconv3x3": 2.0, "convert": 0.0, "zero_tail": 0.0, "lens_derive": 0.0}
 
 
-def check_op(meta, op, before, after, tf32_cut=False):
-    """Compare what op `op` wrote (after: raw bytes once it ran) with its contract evaluated on `before`.  Returns
-    (worst error/bound ratio, list of failure strings naming the op, the element and the values)."""
-    import torch
+LINKED = ("res2_fused", "cam_dense")    # contracts checked link by link: evaluated again on what the kernel stored
+
+
+class Expectation:
+    """an op's contract evaluated on the memory in front of it (expect_op): the fp64 results and error scales, the regions
+    it declares written and the regions it reads"""
+
+    def __init__(self, meta, op, ref, errs, tf32_cut):
+        self.meta, self.op, self.ref, self.errs, self.tf32_cut = meta, op, ref, errs, tf32_cut
+        self.regions = _regions(ref)
+        self.reads = {}
+        for addr, es, shape, strides in ref.reads:
+            base, _ = ref._find(addr)
+            if base in self.regions:
+                self.reads.setdefault(base, []).append(((addr - base) // es, es, shape, strides))
+
+
+def expect_op(meta, op, before, tf32_cut=False):
+    """Evaluate op `op`'s contract on `before` (raw bytes in front of the op) -> Expectation."""
+    tr = op["trace"]
+    ref = RawMemory(meta, before)
+    ref.tf32_cut = tf32_cut and tr["kind"] == "conv" and op["label"].startswith("conv_tc")
+    errs = run_op(ref, tr, meta) or {}
+    return Expectation(meta, op, ref, errs, ref.tf32_cut)
+
+
+def poison(exp, state):
+    """Fill every byte `exp`'s op declares written (outputs, lo twins, side outputs) and its contract does not read with
+    0xFF, in place: NaN in fp32, bf16 and fp16, -1 in the int32 frame counts.  A kernel that leaves a declared output
+    unwritten then leaves NaN behind instead of whatever happened to be there (zeros in fresh memory, which is the right
+    answer for padding rows and ReLU'd tails)."""
+    for base, regs in exp.regions.items():
+        t = state[base]
+        m = _byte_mask(t, regs) & ~_byte_mask(t, exp.reads.get(base, []))
+        t[m] = 255
+    return state
+
+
+def compare_op(exp, before, after):
+    """Compare what exp's op wrote (after: raw bytes once it ran) with the contract; before: the bytes it ran on.  Returns
+    (worst error/bound ratio, list of failure strings naming the op, the element and the values).  NaN is a value like any
+    other: NaN where the contract is NaN agrees, NaN on one side only is an infinite error."""
+    meta, op = exp.meta, exp.op
     tr = op["trace"]
     kind = tr["kind"]
-    ref = RawMemory(meta, before)
-    ref.tf32_cut = tf32_cut and kind == "conv" and op["label"].startswith("conv_tc")
     got = RawMemory(meta, after)
-    ref.links = got
-    errs = run_op(ref, tr, meta) or {}
+    ref, errs = exp.ref, exp.errs
+    if kind in LINKED:          # (its read regions are as they were when exp was made: only declared writes are poisoned)
+        ref = RawMemory(meta, before)
+        ref.links = got
+        errs = run_op(ref, tr, meta) or {}
     fails, worst = [], 0.0
     out_dt = lambda es: ref.act if es == 2 else "fp32"
     for addr, es, shape, strides, hi, side in ref.writes:
         if side:
             continue
-        r = ref.strided(addr, es, shape, strides)
-        g = got.strided(addr, es, shape, strides)
+        r = ref.region(addr, es, shape, strides, False)
+        g = got.region(addr, es, shape, strides, False)
         name = f"{op['label']} [{kind}] @{addr:#x}"
         if hi:                      # lo twin: bit for bit v - tf32_trunc(v) of the stored hi value
-            hv = got.strided(hi, 4, shape, strides).astype(np.float32)
+            hv = got.region(hi, 4, shape, strides, False).astype(np.float32)
             want = (hv - _tf32_trunc(hv)).astype(np.float32)
             bad = np.argwhere(want.view(np.uint32) != g.astype(np.float32).view(np.uint32))
             if len(bad):
@@ -826,23 +891,28 @@ def check_op(meta, op, before, after, tf32_cut=False):
             bound = np.zeros(r.shape)        # frame counts: exact
         else:
             bound = ulp(r, out_dt(es)) + C_KIND[kind] * U32 * np.broadcast_to(np.abs(e), r.shape)
-        d = np.abs(g - r)
-        ratio = np.where(d == 0, 0.0, d / np.where(bound > 0, bound, 1e-300))
-        ratio = np.where(np.isnan(g) & ~np.isnan(r), np.inf, ratio)
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            ratio = np.abs(g - r) / np.where(bound > 0, bound, 1e-300)
+        same = (g == r) | (np.isnan(g) & np.isnan(r))
+        ratio = np.where(same, 0.0, np.where(np.isnan(ratio), np.inf, ratio))   # NaN on one side (or in the bound): infinite
         if ratio.size:
             worst = max(worst, float(ratio.max()))
             if ratio.max() > 1.0:
                 i = np.unravel_index(int(np.argmax(ratio)), ratio.shape)
                 fails.append(f"{name}: {int((ratio > 1).sum())} of {ratio.size} elements out of bound, worst at {i}: "
                              f"got {g[i]!r} want {r[i]!r} bound {bound[i]:.3g} (ratio {ratio[i]:.3g})")
-    regions = _regions(ref)
     for base, _ in ref.allocs:
         diff = before[base] != after[base]
         if not bool(diff.any()):
             continue
-        stray = diff & ~declared_mask(before, regions, base)
+        stray = diff & ~declared_mask(before, exp.regions, base)
         if bool(stray.any()):
             i = int(stray.nonzero()[0])
             fails.append(f"{op['label']} [{kind}]: wrote {int(stray.sum())} bytes outside its declared outputs, first at "
                          f"allocation {base:#x} + {i}")
     return worst, fails
+
+
+def check_op(meta, op, before, after, tf32_cut=False):
+    """expect_op on `before` and compare_op with `after` (no poisoning: `before` is the memory the op ran on)"""
+    return compare_op(expect_op(meta, op, before, tf32_cut), before, after)

@@ -78,14 +78,18 @@ def resnet():
     return meta, states, verdicts
 
 
-def walk(meta, state):
-    """run the plan with the perfect kernel, checking every op; returns the state in front of each op and what the checker
-    said about each (asserted in test_perfect_kernel_passes_every_op)"""
+def walk(meta, state, poisoned=True, stop=None):
+    """run the plan with the perfect kernel, checking every op (on memory poisoned the way tests/test_plan_ops_gpu.py
+    poisons it, unless poisoned=False); returns the state in front of each op and what the checker said about each
+    (asserted in test_perfect_kernel_passes_every_op).  stop: the number of ops to run."""
     states, verdicts = [], []
-    for op in meta["ops"]:
+    for op in meta["ops"][:stop]:
+        exp = pi.expect_op(meta, op, state)
+        if poisoned:
+            state = pi.poison(exp, {a: t.clone() for a, t in state.items()})
         states.append(state)
         after, _ = perfect(meta, state, op["trace"])
-        verdicts.append(pi.check_op(meta, op, state, after))
+        verdicts.append(pi.compare_op(exp, state, after))
         state = after
     return states, verdicts
 
@@ -248,3 +252,84 @@ def test_store_past_cout_is_flagged(ecapa):
     buf[s:s + 32 * 2] ^= 0x5A
     fails = flagged(meta, i, states[i], bad)
     assert any("outside its declared outputs" in f for f in fails)
+
+
+def _rows(tr_view, b, f, t):
+    """byte offset (from the view's address) and length of output row (b, f, t) of a channels-last View"""
+    o = tr_view
+    return ((b * o["F"] + f) * o["T"] + t) * o["ld"] * 2, o["C"] * 2
+
+
+def test_nan_contract_element_does_not_hide_its_region(resnet):
+    """a NaN the contract computes (here from a NaN input element) must not make the rest of the output region a no-op
+    check: an element far out of bound next to it is flagged, and so is a finite value where the contract is NaN"""
+    meta, states, _ = resnet
+    i = first_op(meta, lambda tr, lab: tr["kind"] == "tstats")
+    tr = meta["ops"][i]["trace"]
+    st = {a: t.clone() for a, t in states[i].items()}
+    x = tr["x"]
+    base = max(a for a in st if a <= x["p"])
+    st[base].numpy()[x["p"] - base:x["p"] - base + 2] = np.frombuffer(np.float16(np.nan).tobytes(), np.uint8)
+    good, _ = perfect(meta, st, tr)
+    ob = max(a for a in good if a <= tr["out"])
+    out = good[ob].numpy()[tr["out"] - ob:].view(np.float32)
+    assert np.isnan(out[0]) and np.isfinite(out[1])
+    assert not pi.check_op(meta, meta["ops"][i], st, good)[1]
+    far = {a: t.clone() for a, t in good.items()}
+    far[ob].numpy()[tr["out"] - ob:].view(np.float32)[1] *= 1.01
+    flagged(meta, i, st, far)
+    finite = {a: t.clone() for a, t in good.items()}
+    finite[ob].numpy()[tr["out"] - ob:].view(np.float32)[0] = 0.0
+    flagged(meta, i, st, finite)
+
+
+def test_skipped_padding_rows_fail_only_on_poisoned_memory():
+    """a masked conv3x3 that never writes the zero rows behind an utterance's end passes on zero-initialised memory (zero
+    is the right answer there) and fails once the op's outputs are poisoned in front of it"""
+    meta, blob = trace_of("ResNet34", "fp16", 2, 40, masked=True)
+    n_frames = [40, 13]
+    feats = np.random.default_rng(4).standard_normal((2, 40, 80))
+    i = first_op(meta, lambda tr, lab: tr["kind"] == "conv3x3" and tr["lens"])
+    state = walk(meta, initial_state(meta, blob, feats, n_frames), poisoned=False, stop=i + 1)[0][i]
+    op = meta["ops"][i]
+    tr = op["trace"]
+    o = tr["out"]
+    lens = pi.RawMemory(meta, state).vec(tr["lens"], 2).astype(int)
+    assert lens[1] < o["T"]
+
+    def skip_padding(before, after):
+        bad = {a: t.clone() for a, t in after.items()}
+        base = max(a for a in bad if a <= o["p"])
+        for f in range(o["F"]):
+            for t in range(lens[1], o["T"]):
+                off, n = _rows(o, 1, f, t)
+                s = o["p"] - base + off
+                bad[base].numpy()[s:s + n] = before[base].numpy()[s:s + n]
+        return bad
+    good, _ = perfect(meta, state, tr)
+    assert not pi.check_op(meta, op, state, skip_padding(state, good))[1]
+    exp = pi.expect_op(meta, op, state)
+    poisoned = pi.poison(exp, {a: t.clone() for a, t in state.items()})
+    good, _ = perfect(meta, poisoned, tr)
+    assert not pi.compare_op(exp, poisoned, good)[1]
+    worst, fails = pi.compare_op(exp, poisoned, skip_padding(poisoned, good))
+    assert fails and all(f.startswith(op["label"]) for f in fails), (worst, fails)
+
+
+def test_unwritten_one_row_time_tile_is_flagged():
+    """T = 257 runs the 3x3 kernel in 128-row time tiles, the last one a single row: leaving it unwritten is flagged"""
+    meta, blob = trace_of("ResNet34", "fp16", 1, 257)
+    i = first_op(meta, lambda tr, lab: tr["kind"] == "conv3x3" and tr["out"]["T"] == 257 and "n_mt=1" in lab)
+    feats = np.random.default_rng(5).standard_normal((1, 257, 80))
+    state = walk(meta, initial_state(meta, blob, feats), stop=i + 1)[0][i]
+    tr = meta["ops"][i]["trace"]
+    good, _ = perfect(meta, state, tr)
+    o = tr["out"]
+    bad = {a: t.clone() for a, t in good.items()}
+    base = max(a for a in bad if a <= o["p"])
+    for f in range(o["F"]):
+        off, n = _rows(o, 0, f, 256)
+        s = o["p"] - base + off
+        bad[base].numpy()[s:s + n] = state[base].numpy()[s:s + n]
+    assert not pi.check_op(meta, meta["ops"][i], state, good)[1]
+    flagged(meta, i, state, bad)

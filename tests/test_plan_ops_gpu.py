@@ -6,9 +6,14 @@ time, and after each op:
     reduction length times the statistic's magnitude for the statistics ops; derivations with each contract);
   * containment: no byte of any allocation (weights included) outside the op's declared outputs changed;
   * 3xTF32 lo twins: each written lo twin is v - tf32_trunc(v) of the stored v, bit for bit.
-Errors cannot accumulate from op to op, so a failure names the op, the element and the kernel path (the op label).  After
-the last op the eager embedding must equal the CUDA-graph replay bit for bit, and the real engine's trace must be the
-plan-check engine's trace up to allocation numbering, so the CPU plan-arithmetic tests check the plans the GPU runs.
+Before each op, every element it declares written and its contract does not read is poisoned (NaN; -1 in frame counts), so
+an output the kernel leaves unwritten fails instead of passing on whatever the buffer held; NaN in the contract must be NaN
+in the kernel's output and nowhere else.  Errors cannot accumulate from op to op, so a failure names the op, the element
+and the kernel path (the op label).  After the last op the eager embedding must equal the CUDA-graph replay bit for bit
+(masked plans: replayed with longer frame counts first, then the case's own), the real engine's trace must be the
+plan-check engine's trace up to allocation numbering, so the CPU plan-arithmetic tests check the plans the GPU runs, and
+the plan must reach the ops and geometry branches (tests/plan_edges.py) its case is there for, the SM-count-dependent ones
+included.
 The worst error / bound ratio of each op kind and precision is printed (pytest -s)."""
 import json
 import os
@@ -21,6 +26,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import plan_edges as pe  # noqa: E402
 import plan_interp as pi  # noqa: E402
 from wespeaker_b200.models import from_synthetic  # noqa: E402
 
@@ -52,6 +58,7 @@ CASES = {
     "resnet34_fp16_masked": ("ResNet34", "fp16", 4, 200, [200, 163, 64, 17], {}, {"lens_derive", "zero_tail", "conv3x3"}),
     "campplus_bf16_masked": ("CAMPPlus", "bf16", 4, 200, [200, 163, 64, 17], {}, {"lens_derive", "cam_dense"}),
 }
+CASES.update(pe.EDGE_CASES)     # geometry edges: tile tails, chunk edges, 1-frame utterances (branch keys of plan_edges)
 WORST = {}      # (kind, precision) -> worst error / bound ratio over the cases run
 
 
@@ -105,14 +112,16 @@ def test_plan_ops_match_contracts(case):
     live = pi.device_memory(meta, feats, n_frames)
     torch.cuda.synchronize()
 
-    fails, seen = [], set()
+    fails, seen = [], pe.case_branches(meta["ops"], n_frames)
     for i, op in enumerate(meta["ops"]):
         kind = op["trace"]["kind"]
         seen |= {kind, op["label"].split()[0]} | {w for w in op["label"].split() if w.startswith("bn=")}
+        exp = pi.expect_op(meta, op, live, tf32_cut=prec == "tf32")
+        pi.poison(exp, live)         # what the op declares written and does not read: NaN (-1 in frame counts)
         before = {a: t.clone() for a, t in live.items()}
         m.run_ops(B, T, masked, i, i + 1)
         torch.cuda.synchronize()
-        worst, f = pi.check_op(meta, op, before, live, tf32_cut=prec == "tf32")
+        worst, f = pi.compare_op(exp, before, live)
         WORST[(kind, prec)] = max(WORST.get((kind, prec), 0.0), worst)
         fails += [f"op {i}: {x}" for x in f]
         del before
@@ -123,9 +132,13 @@ def test_plan_ops_match_contracts(case):
     eager = live[max(a for a in live if a <= meta["emb"])]
     off = meta["emb"] - max(a for a in live if a <= meta["emb"])
     eager = eager[off:off + B * m.embed_dim * 4].clone().view(torch.float32).reshape(B, m.embed_dim)
-    if not masked:
+    if masked:      # a replay with other (longer) frame counts first: nothing of it may survive into the next one
+        m.embed_padded(feats.cuda(), [T] * B)
+        graph = m.embed_padded(feats.cuda(), n_frames)
+    else:
         graph = m.embed(feats.cuda())
-        assert torch.equal(eager, graph), f"eager plan differs from its CUDA-graph replay: {(eager - graph).abs().max().item()}"
+    same = torch.equal(eager.view(torch.int32), graph.view(torch.int32))      # bit for bit, NaN for NaN
+    assert same, f"eager plan differs from its CUDA-graph replay: {(eager - graph).abs().nan_to_num(float('inf')).max().item()}"
 
     head, ops, labels = _canonical(meta)
     head_c, ops_c, labels_c = _canonical(meta_check)

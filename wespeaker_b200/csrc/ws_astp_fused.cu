@@ -216,7 +216,7 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
                         const float mean = s1[h] / s0[h];
                         const float var = s2[h] / s0[h] - mean * mean;
                         p.out[(long long)b * 2 * p.C + c] = mean;
-                        p.out[(long long)b * 2 * p.C + p.C + c] = sqrtf(fmaxf(var, p.var_floor));
+                        p.out[(long long)b * 2 * p.C + p.C + c] = sqrtf(var < p.var_floor ? p.var_floor : var);   // torch clamp: NaN stays NaN
                     }
                 }
             }

@@ -93,6 +93,9 @@ int add_conv_taps(ConvSpec& spec, const View& x, int kf, int kt, int dil_f, int 
             v.F = (x.F - pf + stride_f - 1) / stride_f;
             v.T = (x.T - pt + stride_t - 1) / stride_t;
             v.C = x.C;
+            // a parity plane with no rows (the odd plane of a 1-frame or 1-row input): its taps only read padding, and a
+            // zero-extent tensor map cannot be encoded
+            if (v.F < 1 || v.T < 1) continue;
             v.sB = sB;
             v.sF = sF * stride_f;
             v.sT = sT * stride_t;

@@ -431,7 +431,7 @@ __global__ void __launch_bounds__(256) astp_stats_kernel(const void* __restrict_
             const float mean = a1 / a0;
             const float var = a2 / a0 - mean * mean;
             out[(long long)b * 2 * C + cc] = mean;
-            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, var_floor));
+            out[(long long)b * 2 * C + C + cc] = sqrtf(var < var_floor ? var_floor : var);   // torch clamp: NaN stays NaN
         }
     }
 }
@@ -527,7 +527,7 @@ __global__ void __launch_bounds__(512, 2) astp_stats4_kernel(const void* __restr
             const float mean = a1 / a0;
             const float var = a2 / a0 - mean * mean;
             out[(long long)b * 2 * C + cc] = mean;
-            out[(long long)b * 2 * C + C + cc] = sqrtf(fmaxf(var, var_floor));
+            out[(long long)b * 2 * C + C + cc] = sqrtf(var < var_floor ? var_floor : var);   // torch clamp: NaN stays NaN
         }
     }
 }
