@@ -257,14 +257,13 @@ static bool tc2_geometry(const ConvSpec& s, WsTc2Params* q) {
 }
 
 // ---- the persistent tensor-core kernel (ws_gemm_tc2.cu).  cl: CTAs per cluster sharing the weight tile (1, or 2 / 4:
-// ws_tc3_launch).  Returns false with *unsupported set and no error when no N tile suits a cluster of cl >= 2 CTAs (the
-// caller then builds the layer with cl = 1); every other refusal is an error that names the reason.
-static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int cl = 1) {
+// ws_tc3_launch).  Outside when no N tile suits a cluster of cl >= 2 CTAs (the caller then builds the layer with cl = 1);
+// every other refusal is an error that names the reason.
+static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
     const bool pair = cl >= 2;
-    *unsupported = false;
     const WsEpi& e = s.epi;
-    if (s.Cout % 32 != 0) { set_err("tc conv: Cout must be a multiple of 32 (the narrowest N tile)"); return false; }
-    if (e.res != nullptr && e.out2 != nullptr) { set_err("tc conv: a residual and a second output (out2) cannot be combined"); return false; }
+    if (s.Cout % 32 != 0) { set_err("tc conv: Cout must be a multiple of 32 (the narrowest N tile)"); return OpBuild::error; }
+    if (e.res != nullptr && e.out2 != nullptr) { set_err("tc conv: a residual and a second output (out2) cannot be combined"); return OpBuild::error; }
     memset(q, 0, sizeof(*q));
     const int es = ws_esize(s.dt);
     q->has_out2 = e.out2 != nullptr;
@@ -272,12 +271,12 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     q->nsplit = s.split ? 3 : 1;
     if (s.split) {
         if (s.dt != WS_F32 || s.W_lo == nullptr || e.out_lo == nullptr || (q->has_out2 && e.out2_lo == nullptr)) {
-            set_err("tc conv: 3xTF32 needs fp32 activations with lo twins for W / out / out2"); return false;
+            set_err("tc conv: 3xTF32 needs fp32 activations with lo twins for W / out / out2"); return OpBuild::error;
         }
         for (int i = 0; i < s.nsrc; ++i)
-            if (s.src[i].ptr_lo == nullptr) { set_err("tc conv: 3xTF32 source without a lo twin"); return false; }
+            if (s.src[i].ptr_lo == nullptr) { set_err("tc conv: 3xTF32 source without a lo twin"); return OpBuild::error; }
     }
-    if (!tc2_geometry(s, q)) return false;
+    if (!tc2_geometry(s, q)) return OpBuild::error;
     q->nout = (s.split ? 2 : 1) * (q->has_out2 ? 2 : 1);
     const int nstage_bufs = q->nout + (q->has_epin ? 1 : 0);
     const int budget = ws_tc2_max_smem() - 1024;
@@ -321,9 +320,9 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
             if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > max_st ? max_st : n; break; }
         }
     if (bn == 0) {
-        if (pair) *unsupported = true;
-        else set_err("tc conv: no N tile fits in shared memory beside the epilogue staging");
-        return false;
+        if (pair) return OpBuild::outside;
+        set_err("tc conv: no N tile fits in shared memory beside the epilogue staging");
+        return OpBuild::error;
     }
     q->bn = bn; q->nstages = nst;
     q->tiles_n = s.Cout / bn;
@@ -335,9 +334,9 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
         cuuint64_t dims[2] = {(cuuint64_t)s.Ktot, (cuuint64_t)s.Cout};
         cuuint64_t str[1] = {(cuuint64_t)s.Ktot * es};
         cuuint32_t box[2] = {(cuuint32_t)bk_elems, (cuuint32_t)(bn / cl)};   // the rows ONE CTA loads per k-block
-        if (!encode_map(&q->wmap, s.dt, s.W, 2, dims, str, box, q->bk_bytes)) return false;
+        if (!encode_map(&q->wmap, s.dt, s.W, 2, dims, str, box, q->bk_bytes)) return OpBuild::error;
         q->wmap_lo = q->wmap;
-        if (s.split && !encode_map(&q->wmap_lo, s.dt, s.W_lo, 2, dims, str, box, q->bk_bytes)) return false;
+        if (s.split && !encode_map(&q->wmap_lo, s.dt, s.W_lo, 2, dims, str, box, q->bk_bytes)) return OpBuild::error;
     }
     // output / epilogue-input maps: same tile geometry as the A maps over the output positions
     const bool flat = s.dense_pointwise;
@@ -355,14 +354,14 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
         return encode_map(m, s.dt, ptr, 4, dims, str, box, q->panel_bytes);
     };
     int oi = 0;
-    if (!out_map(&q->omap[oi++], e.out, e.out_ld)) return false;
-    if (s.split && !out_map(&q->omap[oi++], e.out_lo, e.out_ld)) return false;
+    if (!out_map(&q->omap[oi++], e.out, e.out_ld)) return OpBuild::error;
+    if (s.split && !out_map(&q->omap[oi++], e.out_lo, e.out_ld)) return OpBuild::error;
     if (q->has_out2) {
-        if (!out_map(&q->omap[oi++], e.out2, e.out2_ld)) return false;
-        if (s.split && !out_map(&q->omap[oi++], e.out2_lo, e.out2_ld)) return false;
-        if (!out_map(&q->imap, e.add2, e.add2_ld)) return false;
+        if (!out_map(&q->omap[oi++], e.out2, e.out2_ld)) return OpBuild::error;
+        if (s.split && !out_map(&q->omap[oi++], e.out2_lo, e.out2_ld)) return OpBuild::error;
+        if (!out_map(&q->imap, e.add2, e.add2_ld)) return OpBuild::error;
     } else if (q->has_epin) {
-        if (!out_map(&q->imap, e.res, e.res_ld)) return false;
+        if (!out_map(&q->imap, e.res, e.res_ld)) return OpBuild::error;
     }
     for (; oi < 4; ++oi) q->omap[oi] = q->omap[0];
     if (!q->has_epin) q->imap = q->omap[0];
@@ -370,7 +369,7 @@ static bool build_tc2(const ConvSpec& s, WsTc2Params* q, bool* unsupported, int 
     if (pair) q->grid = cl * (q->num_tiles < ncl ? q->num_tiles : ncl);
     else q->grid = q->num_tiles < g_num_sms ? q->num_tiles : g_num_sms;
     q->smem_bytes = nst * (128 + bn) * q->bk_bytes + staging_bytes(bn) + 1024;
-    return true;
+    return OpBuild::built;
 }
 
 static bool build_simt(const ConvSpec& s, WsSimtParams* p) {
@@ -401,23 +400,22 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
     if (use_tc >= 3 && (long long)spec.B * spec.F * spec.T >= min_pos) {
         // big layers: clusters of CTAs on adjacent position tiles share the weight tile by TMA multicast
         auto q = std::make_shared<WsTc2Params>();
-        bool unsupported = false;
         // (two CTAs per cluster; WS_TC3_CL=4 takes four on the largest layers)
         static const int cl_env = getenv("WS_TC3_CL") ? atoi(getenv("WS_TC3_CL")) : 2;
         const int cl = (cl_env == 4 && (long long)spec.B * spec.F * spec.T >= 2LL * min_pos) ? 4 : 2;
-        if (build_tc2(spec, q.get(), &unsupported, cl)) {
+        const OpBuild r = build_tc2(spec, q.get(), cl);
+        if (r == OpBuild::built) {
             out->run = [q](cudaStream_t s) { return ws_tc3_launch(q.get(), s); };
             char kn[64];
             snprintf(kn, sizeof kn, "conv_tc3 cl=%d grid=%d bn=%d st=%d", q->cl, q->grid, q->bn, q->nstages);
             label_conv(out, kn, spec);
             return true;
         }
-        if (!unsupported) return false;
+        if (r == OpBuild::error) return false;
     }
     if (use_tc >= 2) {
         auto q = std::make_shared<WsTc2Params>();
-        bool unsupported = false;
-        if (!build_tc2(spec, q.get(), &unsupported)) return false;
+        if (build_tc2(spec, q.get()) != OpBuild::built) return false;
         out->run = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
         label_conv(out, "conv_tc2", spec);
         return true;
@@ -430,14 +428,11 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
     return true;
 }
 
-bool make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
-                  const float* shift, int w8, int dil, PlanOp* op, bool* unsupported, const int* lens) {
-    *unsupported = false;
+OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
+                     const float* shift, int w8, int dil, PlanOp* op, const int* lens) {
     // T > 256: time tiles with a 32-row halo per side cover the chain's receptive field (7 * dil rows) up to dilation 4
-    if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7 || getenv("WS_NO_RES2_FUSED")) {
-        *unsupported = true;
-        return false;
-    }
+    if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7 || getenv("WS_NO_RES2_FUSED"))
+        return OpBuild::outside;
     auto q = std::make_shared<WsRes2Params>();
     memset(q.get(), 0, sizeof(WsRes2Params));
     auto act_map = [&](CUtensorMap* m, const View& v) {
@@ -446,19 +441,19 @@ bool make_res2_op(const View& x, const View& out, const void* W7, const float* b
         cuuint32_t box[3] = {64, 128, 1};
         return encode_map(m, v.dt, v.p, 3, dims, str, box, 128);
     };
-    if (!act_map(&q->xmap, x) || !act_map(&q->omap, out)) return false;
+    if (!act_map(&q->xmap, x) || !act_map(&q->omap, out)) return OpBuild::error;
     {
         cuuint64_t dims[3] = {(cuuint64_t)out.C, (cuuint64_t)out.T, (cuuint64_t)out.B};
         cuuint64_t str[2] = {(cuuint64_t)out.ld * 2, (cuuint64_t)out.T * out.ld * 2};
         cuuint32_t box[3] = {64, 64, 1};
-        if (!encode_map(&q->omap64, out.dt, out.p, 3, dims, str, box, 128)) return false;
+        if (!encode_map(&q->omap64, out.dt, out.p, 3, dims, str, box, 128)) return OpBuild::error;
     }
     q->ntile = x.T <= 256 ? 1 : (x.T + 191) / 192;
     {
         cuuint64_t dims[2] = {(cuuint64_t)(3 * w8), (cuuint64_t)(7 * w8)};
         cuuint64_t str[1] = {(cuuint64_t)(3 * w8) * 2};
         cuuint32_t box[2] = {64, (cuuint32_t)w8};
-        if (!encode_map(&q->wmap, x.dt, W7, 2, dims, str, box, 128)) return false;
+        if (!encode_map(&q->wmap, x.dt, W7, 2, dims, str, box, 128)) return OpBuild::error;
     }
     q->x = x.p; q->ld = x.ld; q->bias = bias; q->scale = scale; q->shift = shift; q->lens = lens;
     q->B = x.B; q->T = x.T; q->w8 = w8; q->dil = dil; q->dtype = x.dt;
@@ -474,36 +469,32 @@ bool make_res2_op(const View& x, const View& out, const void* W7, const float* b
     snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", x.B, x.T, x.C);
     op->label = buf;
     op->flops = 2.0 * x.B * x.T * 7.0 * 3.0 * (x.C / 8.0) * (x.C / 8.0);
-    return true;
+    return OpBuild::built;
 }
 
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, bool* unsupported,
-                  const int* lens) {
-    *unsupported = false;
+OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, const int* lens) {
     if (x.dt == WS_F32 || h.dt != x.dt || x.C % 128 != 0 || h.C != 128 || h.ld != 128 || x.F != 1 || h.F != 1 || h.T != x.T ||
-        h.B != x.B || getenv("WS_NO_ASTP_FUSED")) {
-        *unsupported = true;
-        return false;
-    }
+        h.B != x.B || getenv("WS_NO_ASTP_FUSED"))
+        return OpBuild::outside;
     auto q = std::make_shared<WsAstpParams>();
     memset(q.get(), 0, sizeof(WsAstpParams));
     {
         cuuint64_t dims[3] = {128, (cuuint64_t)h.T, (cuuint64_t)h.B};
         cuuint64_t str[2] = {128 * 2, (cuuint64_t)h.T * 128 * 2};
         cuuint32_t box[3] = {64, 256, 1};
-        if (!encode_map(&q->hmap, h.dt, h.p, 3, dims, str, box, 128)) return false;
+        if (!encode_map(&q->hmap, h.dt, h.p, 3, dims, str, box, 128)) return OpBuild::error;
     }
     {
         cuuint64_t dims[2] = {128, (cuuint64_t)x.C};
         cuuint64_t str[1] = {128 * 2};
         cuuint32_t box[2] = {64, 128};
-        if (!encode_map(&q->wmap, x.dt, W2, 2, dims, str, box, 128)) return false;
+        if (!encode_map(&q->wmap, x.dt, W2, 2, dims, str, box, 128)) return OpBuild::error;
     }
     {
         cuuint64_t dims[3] = {(cuuint64_t)x.C, (cuuint64_t)x.T, (cuuint64_t)x.B};
         cuuint64_t str[2] = {(cuuint64_t)x.ld * 2, (cuuint64_t)x.T * x.ld * 2};
         cuuint32_t box[3] = {128, 128, 1};
-        if (!encode_map(&q->xmap, x.dt, x.p, 3, dims, str, box, 0)) return false;
+        if (!encode_map(&q->xmap, x.dt, x.p, 3, dims, str, box, 0)) return OpBuild::error;
     }
     q->x = x.p; q->x_ld = x.ld; q->out = stats; q->B = x.B; q->T = x.T; q->C = x.C; q->dtype = x.dt; q->lens = lens;
     q->var_floor = var_floor;
@@ -524,7 +515,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
     q->grid = (int)(units < sms ? units : sms);
     if (getenv("WS_ASTP_PROF")) {   // tuning aid: synchronous launch + per-role wait-cycle summary on stderr
         long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("astp: prof buffer"); return false; }
+        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("astp: prof buffer"); return OpBuild::error; }
         q->prof = prof;
         op->run = [q](cudaStream_t s) -> const char* {
             cudaMemsetAsync(q->prof, 0, (size_t)q->grid * 16 * 8, s);
@@ -545,7 +536,7 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
             return nullptr;
         };
         op->label = "astp_fused (profiled)";
-        return true;
+        return OpBuild::built;
     }
     op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
     if (plan_trace_mode())
@@ -555,21 +546,18 @@ bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, fl
     snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);
     op->label = buf;
     op->flops = 2.0 * x.B * x.T * 128.0 * x.C;
-    return true;
+    return OpBuild::built;
 }
 
-bool make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
-                     PlanOp* op, bool* unsupported, int stride_f, int stride_t, const int* lens) {
-    *unsupported = false;
+OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
+                        PlanOp* op, int stride_f, int stride_t, const int* lens) {
     const int Cin = x.C, Cout = out.C, Tin = x.T, Fin = x.F, B = x.B;
     const int F = (Fin + 2 - 3) / stride_f + 1, T = (Tin + 2 - 3) / stride_t + 1;   // output extents
     auto chan_ok = [](int c) { return c == 32 || c == 64 || c == 128; };
     if (x.dt == WS_F32 || out.dt != x.dt || !chan_ok(Cin) || !chan_ok(Cout) || out.B != B || out.F != F || out.T != T ||
         (stride_f != 1 && stride_f != 2) || (stride_t != 1 && stride_t != 2) || T < 1 || F < 1 || (x.ld * 2) % 16 != 0 || (out.ld * 2) % 16 != 0 || (res && (res->ld * 2) % 16 != 0) ||
-        getenv("WS_NO_CONV3X3")) {
-        *unsupported = true;
-        return false;
-    }
+        getenv("WS_NO_CONV3X3"))
+        return OpBuild::outside;
     auto q = std::make_shared<WsC3Params>();
     memset(q.get(), 0, sizeof(WsC3Params));
     q->B = B; q->F = F; q->T = T; q->Cin = Cin; q->Cout = Cout; q->dtype = x.dt;
@@ -640,7 +628,7 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
         const bool pref256 = 2 * ((T + 255) / 256) <= (T + 127) / 128;
         ok = pref256 ? (try_geom(false, 256, 2) || try_geom(false, 128, 1)) : (try_geom(false, 128, 1) || try_geom(false, 256, 2));
     }
-    if (!ok) { *unsupported = true; return false; }
+    if (!ok) return OpBuild::outside;
     q->total_steps = q->n_nt * q->n_tt * q->n_bg * F;
     const int sms = ws_num_sms();
     q->grid = q->total_steps < sms ? q->total_steps : sms;
@@ -650,35 +638,35 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
         cuuint64_t de[4] = {(cuuint64_t)Cin, (cuuint64_t)((Tin + 1) / 2), (cuuint64_t)Fin, (cuuint64_t)B};
         cuuint64_t dod[4] = {(cuuint64_t)Cin, (cuuint64_t)std::max(1, Tin / 2), (cuuint64_t)Fin, (cuuint64_t)B};
         cuuint32_t be[4] = {(cuuint32_t)q->kc, (cuuint32_t)q->tb, 1, 1}, bo[4] = {(cuuint32_t)q->kc, (cuuint32_t)(q->tb + 1), 1, 1};
-        if (Tin < 2) { *unsupported = true; return false; }
-        if (!encode_map(&q->amap, x.dt, x.p, 4, de, str, be, q->row_bytes)) return false;
-        if (!encode_map(&q->amap_tail, x.dt, (const char*)x.p + (size_t)x.ld * 2, 4, dod, str, bo, q->row_bytes)) return false;
+        if (Tin < 2) return OpBuild::outside;
+        if (!encode_map(&q->amap, x.dt, x.p, 4, de, str, be, q->row_bytes)) return OpBuild::error;
+        if (!encode_map(&q->amap_tail, x.dt, (const char*)x.p + (size_t)x.ld * 2, 4, dod, str, bo, q->row_bytes)) return OpBuild::error;
     } else {
         cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Tin, (cuuint64_t)Fin, (cuuint64_t)B};
         cuuint64_t str[3] = {(cuuint64_t)x.ld * 2, (cuuint64_t)Tin * x.ld * 2, (cuuint64_t)Fin * Tin * x.ld * 2};
         cuuint32_t box[4] = {(cuuint32_t)q->kc, (cuuint32_t)(q->single_box ? q->P : 128), 1, (cuuint32_t)q->nb};
-        if (!encode_map(&q->amap, x.dt, x.p, 4, dims, str, box, q->row_bytes)) return false;
+        if (!encode_map(&q->amap, x.dt, x.p, 4, dims, str, box, q->row_bytes)) return OpBuild::error;
         cuuint32_t boxt[4] = {(cuuint32_t)q->kc, 2, 1, 1};
-        if (!encode_map(&q->amap_tail, x.dt, x.p, 4, dims, str, boxt, q->row_bytes)) return false;
+        if (!encode_map(&q->amap_tail, x.dt, x.p, 4, dims, str, boxt, q->row_bytes)) return OpBuild::error;
     }
     {
         cuuint64_t dims[2] = {(cuuint64_t)(9 * Cin), (cuuint64_t)Cout};
         cuuint64_t str[1] = {(cuuint64_t)(9 * Cin) * 2};
         cuuint32_t box[2] = {(cuuint32_t)q->kc, (cuuint32_t)q->N};
-        if (!encode_map(&q->wmap, x.dt, W, 2, dims, str, box, q->row_bytes)) return false;
+        if (!encode_map(&q->wmap, x.dt, W, 2, dims, str, box, q->row_bytes)) return OpBuild::error;
     }
     {
         cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)F, (cuuint64_t)B};
         cuuint64_t str[3] = {(cuuint64_t)out.ld * 2, (cuuint64_t)T * out.ld * 2, (cuuint64_t)F * T * out.ld * 2};
         cuuint32_t box[4] = {(cuuint32_t)q->panel_cols, (cuuint32_t)(q->case_b ? q->P : 128), 1, (cuuint32_t)(q->case_b ? q->nb : 1)};
-        if (!encode_map(&q->omap, x.dt, out.p, 4, dims, str, box, q->panel_bytes)) return false;
+        if (!encode_map(&q->omap, x.dt, out.p, 4, dims, str, box, q->panel_bytes)) return OpBuild::error;
     }
     q->rmap = q->omap;
     if (res) {
         cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)F, (cuuint64_t)B};
         cuuint64_t str[3] = {(cuuint64_t)res->ld * 2, (cuuint64_t)T * res->ld * 2, (cuuint64_t)F * T * res->ld * 2};
         cuuint32_t box[4] = {(cuuint32_t)q->panel_cols, (cuuint32_t)(q->case_b ? q->P : 128), 1, (cuuint32_t)(q->case_b ? q->nb : 1)};
-        if (!encode_map(&q->rmap, x.dt, res->p, 4, dims, str, box, q->panel_bytes)) return false;
+        if (!encode_map(&q->rmap, x.dt, res->p, 4, dims, str, box, q->panel_bytes)) return OpBuild::error;
     }
     q->res = res ? res->p : nullptr;
     q->res_ld = res ? res->ld : 0;
@@ -697,7 +685,7 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
                     "," + tp("lens", lens) + "}";
     if (getenv("WS_C3_PROF")) {   // tuning aid: synchronous launch + per-role wait-cycle summary on stderr
         long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("conv3x3: prof buffer"); return false; }
+        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("conv3x3: prof buffer"); return OpBuild::error; }
         cudaMemset(prof, 0, (size_t)q->grid * 16 * 8);
         q->prof = prof;
         op->run = [q](cudaStream_t s) -> const char* {
@@ -718,10 +706,10 @@ bool make_conv3x3_op(const View& x, const View& out, const void* W, const float*
             fprintf(stderr, "\n");
             return nullptr;
         };
-        return true;
+        return OpBuild::built;
     }
     op->run = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
-    return true;
+    return OpBuild::built;
 }
 
 extern "C" int ws_cam_smem_bytes(int nmt, int nstages);
@@ -749,14 +737,10 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
     return true;
 }
 
-bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, bool* unsupported,
-                       const int* lens) {
-    *unsupported = false;
+OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, const int* lens) {
     const int T = X.T, B = X.B;
-    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0 || getenv("WS_NO_CAM_FUSED")) {
-        *unsupported = true;
-        return false;
-    }
+    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0 || getenv("WS_NO_CAM_FUSED"))
+        return OpBuild::outside;
     auto q = std::make_shared<WsCamParams>();
     memset(q.get(), 0, sizeof(WsCamParams));
     q->layers = layers_dev; q->l0 = l0; q->l1 = l1; q->lens = lens;
@@ -764,21 +748,21 @@ bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int 
     q->hrows = 16 + 128 * q->nmt;
     int nst = 6;
     while (nst >= 2 && ws_cam_smem_bytes(q->nmt, nst) > ws_cam_max_smem()) --nst;
-    if (nst < 2) { *unsupported = true; return false; }
+    if (nst < 2) return OpBuild::outside;
     q->nstages = nst;
     q->smem_bytes = ws_cam_smem_bytes(q->nmt, nst);
     q->grid = B;
     cuuint64_t dims[3] = {(cuuint64_t)X.C, (cuuint64_t)T, (cuuint64_t)B};
     cuuint64_t str[2] = {(cuuint64_t)X.ld * 2, (cuuint64_t)T * X.ld * 2};
     cuuint32_t boxx[3] = {64, 128, 1}, boxo[3] = {32, 128, 1};
-    if (!encode_map(&q->xmap, X.dt, X.p, 3, dims, str, boxx, 128)) return false;
-    if (!encode_map(&q->omap, X.dt, X.p, 3, dims, str, boxo, 64)) return false;
+    if (!encode_map(&q->xmap, X.dt, X.p, 3, dims, str, boxx, 128)) return OpBuild::error;
+    if (!encode_map(&q->omap, X.dt, X.p, 3, dims, str, boxo, 64)) return OpBuild::error;
     char buf[160];
     snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
     op->label = buf;
     if (getenv("WS_CAM_PROF")) {   // tuning aid: synchronous launch + phase timestamps (cycles since kernel start) of CTA 0
         long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, 16 * 8) != cudaSuccess) { set_err("cam_dense: prof buffer"); return false; }
+        if (cudaMalloc((void**)&prof, 16 * 8) != cudaSuccess) { set_err("cam_dense: prof buffer"); return OpBuild::error; }
         cudaMemset(prof, 0, 16 * 8);
         q->prof = prof;
         op->run = [q](cudaStream_t s) -> const char* {
@@ -794,10 +778,10 @@ bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int 
             fprintf(stderr, "\n");
             return nullptr;
         };
-        return true;
+        return OpBuild::built;
     }
     op->run = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
-    return true;
+    return OpBuild::built;
 }
 
 }  // namespace ws
@@ -839,11 +823,11 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
         // halo-resident 3x3 kernel: act(conv + bias [+ res]); with a residual the activation is act2, else act1 (or act2)
         View r = o;
         r.p = const_cast<void*>(d->res); r.ld = d->res_ld;
-        bool unsupported = false;
         const int a = d->act1 | d->act2;   // one of them is set, or both to the same (idempotent) activation
-        if (make_conv3x3_op(x, o, d->w, d->bias, d->res ? &r : nullptr, a == WS_ACT_RELU20 ? 2 : (a != 0 ? 1 : 0), &op, &unsupported, d->stride_f,
-                            d->stride_t)) done = true;
-        else if (!unsupported) return 1;
+        const OpBuild made = make_conv3x3_op(x, o, d->w, d->bias, d->res ? &r : nullptr, a == WS_ACT_RELU20 ? 2 : (a != 0 ? 1 : 0), &op,
+                                             d->stride_f, d->stride_t);
+        if (made == OpBuild::error) return 1;
+        done = made == OpBuild::built;
     }
     if (!done && !make_conv_op(s, d->use_tc >= 4 ? 3 : d->use_tc, &op)) return 1;
     const char* m = op.run((cudaStream_t)stream);

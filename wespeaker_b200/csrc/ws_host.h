@@ -122,35 +122,37 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out);  // 0 FFMA, 2 
 
 void fill_epi_out(WsEpi& e, const View& out);
 
+// What a fused-op constructor made of a request: the op (built); nothing, because the shape is outside its kernel's envelope
+// (outside: no error is set, the caller builds the layer another way); or nothing, because of an error (set_err says which).
+enum class OpBuild { built, outside, error };
+
 // Fused Res2 chain over a whole SE_Res2Block stage (7 dilated k=3 convs on w8-channel groups, ecapa_tdnn.py:29-78).
 // x: block input (B,1,T,8*w8), out: block output buffer (groups 0..6 are written).  W7: [7*w8][3*w8] packed weights in
-// the activation dtype; bias/scale/shift: [7][w8] fp32.  Returns false with *unsupported=true when the shape/dtype is
-// outside the fused kernel's envelope (16-bit activations, w8 in {64,128}, T <= 256).
-bool make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
-                  const float* shift, int w8, int dil, PlanOp* op, bool* unsupported, const int* lens = nullptr);
+// the activation dtype; bias/scale/shift: [7][w8] fp32.  Outside the fused kernel's envelope: fp32 activations, w8 not in
+// {64,128}, dilation > 4 with T > 256.
+OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
+                     const float* shift, int w8, int dil, PlanOp* op, const int* lens = nullptr);
 
 // Fused ASTP tail (ws_astp_fused.cu): x = frame-level features (B,1,T,C), h = the attention's hidden layer (B,1,T,128), W2 =
 // linear2 weight [C][128] in the activation dtype, stats = fp32 [B][2C] (weighted mean, std = sqrt(max(var, var_floor))).
-// linear2's bias cancels in the softmax over time and is not needed.  *unsupported = true outside the envelope (fp32
-// activations, C % 128, hidden width != 128).
-bool make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, bool* unsupported,
-                  const int* lens = nullptr);
+// linear2's bias cancels in the softmax over time and is not needed.  Outside the envelope: fp32 activations, C % 128,
+// hidden width != 128.
+OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op,
+                     const int* lens = nullptr);
 
 // Halo-resident 3x3 pad-1 conv (ws_conv3x3.cu), strides 1 or 2 per axis: out = act(conv(x, W) + bias [+ res]).  x/out/res:
 // channels-last 16-bit views (out / res with the strided extents); W: [Cout][9*Cin] tap-major in the activation dtype; relu: 0 none,
-// 1 ReLU, 2 Hardtanh(0, 20).  Returns false with
-// *unsupported = true when the shape is outside the kernel's envelope (the caller then uses make_conv_op).
-bool make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
-                     PlanOp* op, bool* unsupported, int stride_f = 1, int stride_t = 1, const int* lens = nullptr);
+// 1 ReLU, 2 Hardtanh(0, 20).  Outside the kernel's envelope, the caller uses make_conv_op.
+OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
+                        PlanOp* op, int stride_f = 1, int stride_t = 1, const int* lens = nullptr);
 
 // Fused CAM++ dense layers (ws_cam_dense.cu).  cam_layer_fill builds one host-side layer descriptor (weights are device
 // pointers in the activation dtype: W1 [128][cin] with BN2 folded, Wl [32][3*128] tap-major; everything else fp32 device
 // arrays).  make_cam_dense_op launches layers [l0, l1) of a device-resident descriptor array over the concat buffer X
-// (B,1,T,Cmax).  *unsupported = true when the shape is outside the kernel's envelope (T > 512, fp32 activations).
+// (B,1,T,Cmax).  Outside the kernel's envelope: T > 512, fp32 activations.
 bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const float* bn1_scale, const float* bn1_shift,
                     const float* bias2, const float* w1c_t, const float* b1c, const float* w2c_t, const float* b2c, int cin,
                     int dil);
-bool make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, bool* unsupported,
-                       const int* lens = nullptr);
+OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, const int* lens = nullptr);
 
 }  // namespace ws
