@@ -126,6 +126,12 @@ int ws_resample(const void* wav_dev, int wav_is_i16, long long wav_ld, int n_in,
                 float* out_dev, long long out_ld, void* stream);
 int ws_fbank(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B, const char* window_type,
              int apply_cmn, float* feats_dev, void* stream);
+/* Ragged fbank, one launch: row b = n_frames_dev[b] frames starting at sample offsets_dev[b] of the flat buffer wav_dev
+ * (total_samples samples); feats_dev fp32 [B][max_frames][80], rows behind n_frames_dev[b] are not written.  No CMN.  A frame
+ * depends on its own 400 samples only, so a long segment may be presented as several rows (row k starting 160 * C * k samples
+ * later) with identical results.  The caller guarantees offsets_dev[b] + 160 * (n_frames_dev[b] - 1) + 400 <= total_samples. */
+int ws_fbank_ragged(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
+                    const int* n_frames_dev, int max_frames, int B, const char* window_type, float* feats_dev, void* stream);
 
 /* ---- generic fused conv operator (channels-last), the building block of the engine; exported for parity tests
  *      against torch conv1d/conv2d.  Replaces Conv1dReluBn (ecapa_tdnn.py:85-106), BasicBlock convs
@@ -239,6 +245,26 @@ int ws_score_cohort_stats(const double* unit_emb_dev, long long N, const double*
 int ws_score_asnorm(const double* scores_dev, const long long* enroll_idx_dev, const long long* test_idx_dev,
                     long long ntrials, const double* enroll_mean_dev, const double* enroll_std_dev,
                     const double* test_mean_dev, const double* test_std_dev, double* out_dev, void* stream);
+
+/* ---- diarization around the engine's forward (wespeaker/cli/speaker.py:213-270): sub-segment windows and the spectral
+ *      clusterer's Laplacian.  All pointers are device pointers.  Tables index the rows of a flat [total_rows][feat_dim] fp32
+ *      feature buffer; an entry that is not inside [0, total_rows) or has len <= 0 is never read and its output is zeros. */
+#define WS_DIAR_MAX_M 16384
+/* out[s][c] = mean over rows [row0[s], row0[s] + len[s]) of feats[.][c] (the segment CMN of diar/make_fbank.py:85-86) */
+int ws_diar_col_means(const float* feats_dev, long long total_rows, int feat_dim, const int* row0_dev, const int* len_dev,
+                      int S, float* out_dev /* [S][feat_dim] */, void* stream);
+/* diar/extract_emb.py:55-83 + cli/speaker.py:110-112: out[w][r][c] = feats[row0[w] + (r mod len[w])][c] - mean_w[c], r in
+ * [0, window_fs).  mean_w = the mean of the window_fs tiled rows when subseg_cmn != 0; else seg_mean[seg_of[w]] when
+ * seg_mean_dev ([S][feat_dim]) is given, else 0.  feat_dim <= 256. */
+int ws_diar_windows(const float* feats_dev, long long total_rows, int feat_dim, const int* row0_dev, const int* len_dev,
+                    int W, int window_fs, int subseg_cmn, const float* seg_mean_dev, const int* seg_of_dev, int S,
+                    float* out_dev /* [W][window_fs][feat_dim] */, void* stream);
+/* diar/spectral_clusterer.py:35-56 on m unit rows (ws_score_unit_rows): cosine affinity, the keep_per_row largest of each row
+ * (the diagonal competes, as there) set to 1 and the rest to 0 - ties at the boundary go to the lowest columns -, symmetrised,
+ * diagonal cleared, lap = diag(row sums) - matrix in fp64.  work_dev: fp32 scratch of work_rows x m cosine tiles; adj_dev:
+ * m x m bytes of scratch.  m > WS_DIAR_MAX_M is refused. */
+int ws_diar_laplacian(const double* unit_dev, long long m, int D, long long keep_per_row, float* work_dev,
+                      long long work_rows, unsigned char* adj_dev, double* lap_dev /* [m][m] */, void* stream);
 
 #ifdef __cplusplus
 }

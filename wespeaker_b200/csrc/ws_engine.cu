@@ -465,6 +465,22 @@ int ws_fbank(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples
     return fbank_into(t, wav_dev, wav_is_i16, wav_ld, nsamples, B, apply_cmn, feats_dev, (cudaStream_t)stream);
 }
 
+int ws_fbank_ragged(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
+                    const int* n_frames_dev, int max_frames, int B, const char* window_type, float* feats_dev, void* stream) {
+    if (!wav_dev || !offsets_dev || !n_frames_dev || !feats_dev || B < 0 || max_frames < 0 || total_samples < 0) {
+        set_err("ws_fbank_ragged: bad argument"); return 1;
+    }
+    if (B > 65535) { set_err("ws_fbank_ragged: more than 65535 rows in one launch"); return 1; }
+    int dev = 0;
+    WS_CK(cudaGetDevice(&dev));
+    const FbankTables* t = fbank_tables(fbank_holder(dev), window_type);
+    if (!t) return 1;
+    // the launcher's size check is per row there; rows are placed by the caller here, which vouches for them
+    WS_CKS(ws_launch_fbank(wav_dev, wav_is_i16, 0, max_frames > 0 ? (max_frames - 1) * 160 + 400 : 0, B, max_frames, t->window,
+                           t->melw, t->melstart, t->mellen, t->maxlen, feats_dev, (cudaStream_t)stream, offsets_dev, n_frames_dev));
+    return 0;
+}
+
 // ---- resampling (torchaudio.transforms.Resample defaults: sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99)
 namespace {
 struct ResampleTaps { float* dev = nullptr; int of = 0, nf = 0, width = 0; };

@@ -13,6 +13,7 @@
 #include "../../include/wespeaker_b200.h"
 #include "ws_host.h"
 #include "ws_kernels.cuh"
+#include "ws_select.cuh"
 
 using namespace ws;
 
@@ -60,48 +61,14 @@ __global__ void __launch_bounds__(256) cos_trials_kernel(const double* __restric
     if (lane == 0) out[r] = acc;
 }
 
-__device__ __forceinline__ uint32_t order_key(float v) {   // larger float <=> larger key
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 // one block per row of the score tile: mean / population std of the top_n largest of M scores
 __global__ void __launch_bounds__(256) topn_stats_kernel(const float* __restrict__ scores, long long M, int top_n,
                                                          double* __restrict__ mean_out, double* __restrict__ std_out) {
-    __shared__ unsigned hist[256];
-    __shared__ uint32_t s_prefix;
-    __shared__ unsigned s_need;
     __shared__ double red[2][8];
     const float* row = scores + (long long)blockIdx.x * M;
     const int tid = threadIdx.x;
-    if (tid == 0) { s_prefix = 0u; s_need = (unsigned)top_n; }
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 24 - 8 * pass;
-        hist[tid] = 0u;
-        __syncthreads();
-        const uint32_t prefix = s_prefix;
-        const uint32_t hi_mask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-        for (long long j = tid; j < M; j += 256) {
-            const uint32_t k = order_key(row[j]);
-            if ((k & hi_mask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned need = s_need;
-            int b = 255;
-            for (; b > 0; --b) {
-                if (hist[b] >= need) break;
-                need -= hist[b];
-            }
-            s_need = need;                       // how many of the selected bin (finally: of the threshold value) to take
-            s_prefix = prefix | ((uint32_t)b << shift);
-        }
-        __syncthreads();
-    }
-    const uint32_t thr_key = s_prefix;
+    unsigned n_ties;
+    const uint32_t thr_key = radix_select_kth(row, M, (unsigned)top_n, &n_ties);
     const double thr = (double)key_value(thr_key);
     double s1 = 0.0, s2 = 0.0;
     for (long long j = tid; j < M; j += 256) {
@@ -114,7 +81,7 @@ __global__ void __launch_bounds__(256) topn_stats_kernel(const float* __restrict
     if (tid == 0) {
         double a = 0.0, b2 = 0.0;
         for (int i = 0; i < 8; ++i) { a += red[0][i]; b2 += red[1][i]; }
-        const double ties = (double)s_need;
+        const double ties = (double)n_ties;
         a += ties * thr; b2 += ties * thr * thr;
         const double n = (double)top_n;
         const double mean = a / n;

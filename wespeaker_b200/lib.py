@@ -94,6 +94,8 @@ _PROTOS = {
     "ws_fbank_num_frames": (C.c_int, [C.c_int]),
     "ws_fbank": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_void_p,
                            C.c_void_p]),
+    "ws_fbank_ragged": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_char_p,
+                                  C.c_void_p, C.c_void_p]),
     "ws_conv": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     "ws_simam": (C.c_int, [C.POINTER(SimamDesc), C.c_void_p]),
     "ws_dwconv": (C.c_int, [C.POINTER(DwConvDesc), C.c_void_p]),
@@ -112,6 +114,11 @@ _PROTOS = {
                                         C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ws_score_asnorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ws_diar_col_means": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ws_diar_windows": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "ws_diar_laplacian": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_PROTOS.keys())
 

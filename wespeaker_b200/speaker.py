@@ -1,7 +1,7 @@
 """`Speaker` API mirror (seam B3, SURVEY.md §8b) of `wespeaker/cli/speaker.py:39-178,296-335` — the
-embedding-extraction methods only (VAD, diarization and the model hub are out of scope).  fbank, CMN and the
-model forward all run on the GPU through the C ABI; WAV decoding uses the stdlib ``wave`` module so that no
-torchaudio IO backend is needed."""
+embedding-extraction methods, and `:76-88,213-289` — diarization with the speech segments given by the caller (VAD and the
+model hub are out of scope).  fbank, CMN, sub-segmentation and the model forward all run on the GPU through the C ABI; WAV
+decoding uses the stdlib ``wave`` module so that no torchaudio IO backend is needed."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ import torch
 import yaml
 
 from .frontend import fbank_batch
-from . import frontend
+from . import diar, frontend
 from .models import get_speaker_model, load_checkpoint
 
 
@@ -57,6 +57,7 @@ class Speaker:
             else torch.device("cpu")
         self.wavform_norm = False
         self.window_type = "hamming"
+        self.set_diarization_params(batch_size=256)
 
     def set_wavform_norm(self, wavform_norm: bool):
         self.wavform_norm = wavform_norm
@@ -75,6 +76,16 @@ class Speaker:
     def set_device(self, device: str):
         self.device = torch.device(device)
         self.model = self.model.to(self.device)
+
+    def set_diarization_params(self, min_duration: float = 0.255, window_secs: float = 1.5, period_secs: float = 0.75,
+                               frame_shift: int = 10, batch_size: int = 32, subseg_cmn: bool = True):
+        """`cli/speaker.py:76-88`.  batch_size bounds the windows per engine launch; the result does not depend on it."""
+        self.diar_min_duration = min_duration
+        self.diar_window_secs = window_secs
+        self.diar_period_secs = period_secs
+        self.diar_frame_shift = frame_shift
+        self.diar_batch_size = batch_size
+        self.diar_subseg_cmn = subseg_cmn
 
     def compute_features(self, wavform: torch.Tensor, sample_rate: int = 16000, cmn: bool = True):
         """`cli/speaker.py:90-106`: (C,N) waveform -> (1,T,80) features on the GPU."""
@@ -156,6 +167,40 @@ class Speaker:
                 best_score = score
                 best_name = name
         return {"name": best_name, "confidence": best_score}
+
+    def diarize(self, audio_path: str, utt: str = "unk", segments=None):
+        """`cli/speaker.py:213-270` with the speech segments [(begin_s, end_s)] given instead of found by VAD, and the
+        reference's spectral clusterer in place of umap + hdbscan: -> [(utt, begin_s, end_s, label)].  subseg_cmn=False
+        means no CMN at all, as there."""
+        if segments is None:
+            raise NotImplementedError("silero VAD is out of scope: pass the speech segments [(begin_s, end_s)]")
+        if len(segments) == 0:
+            return []
+        pcm, sample_rate = read_wav(audio_path, normalize=False)
+        pcm = pcm[:1].to(self._cuda_device())
+        if sample_rate != 16000:
+            pcm, sample_rate = frontend.resample(pcm, sample_rate, 16000), 16000
+        subsegs, embeddings = diar.extract_subsegment_embeddings(
+            self.model, pcm, segments, sample_rate, self.diar_window_secs, self.diar_period_secs, self.diar_frame_shift,
+            self.diar_min_duration, self.diar_batch_size, "window" if self.diar_subseg_cmn else "none", self.window_type)
+        labels = diar.cluster(embeddings)
+        subseg2label = [(*diar.subseg_times(s, self.diar_frame_shift), int(la)) for s, la in zip(subsegs, labels)]
+        return diar.merge_segments({utt: subseg2label})
+
+    def diarize_list(self, scp_path: str, segments_path: str):
+        """`cli/speaker.py:272-281`; segments_path is the recipe's `segments` file (`seg utt begin_s end_s`)."""
+        utt_to_segments = diar.read_segments(segments_path)
+        utts, segment2labels = [], []
+        with open(scp_path, "r", encoding="utf-8") as read_scp:
+            for line in read_scp:
+                utt, wav_path = line.strip().split()
+                utts.append(utt)
+                segs = [(b, e) for _, b, e in utt_to_segments.get(utt, [])]
+                segment2labels.append(self.diarize(wav_path, utt, segs))
+        return utts, segment2labels
+
+    def make_rttm(self, merged_segment_to_labels, outfile: str):
+        diar.make_rttm(merged_segment_to_labels, outfile)
 
 
 def load_model(model_dir: str, precision: str | None = None) -> Speaker:
