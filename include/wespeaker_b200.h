@@ -266,6 +266,30 @@ int ws_diar_windows(const float* feats_dev, long long total_rows, int feat_dim, 
 int ws_diar_laplacian(const double* unit_dev, long long m, int D, long long keep_per_row, float* work_dev,
                       long long work_rows, unsigned char* adj_dev, double* lap_dev /* [m][m] */, void* stream);
 
+/* ---- verification metrics (wespeaker/utils/score_metrics.py:58-116 behind bin/compute_metrics.py and bin/compute_det.py):
+ *      the rbst miss / false-alarm curves over the trials in the stable ascending order of (score, trial line), the EER
+ *      crossing and the minimum detection cost per operating point.  -0.0 == +0.0 (ordered by line), +-inf are ordered. */
+#define WS_METRICS_MAX_POINTS 16
+#define WS_METRICS_MAX_N 2147483647LL
+/* status word bits (out[7]): refusals only the data can reveal; with any of the first three set nothing but out[7] is written */
+#define WS_METRICS_NAN_SCORE 1u
+#define WS_METRICS_BAD_LABEL 2u     /* a label other than 0 or 1 */
+#define WS_METRICS_EMPTY_CLASS 4u   /* no target or no non-target trial */
+#define WS_METRICS_NO_X2 8u         /* fnr - fpr is >= 0 everywhere: the EER has no lower crossing point */
+/* device workspace for n trials; 0 when n is outside [1, WS_METRICS_MAX_N] */
+size_t ws_metrics_work_bytes(long long n);
+/* scores_dev fp64 [n], labels_dev uint8 [n] (1 target, 0 non-target); p_target / c_miss / c_fa: HOST arrays of n_points
+ * (1..16) operating points, 0 < p_target < 1, finite costs >= 0.  out_dev fp64 [8 + n_points] = fnr(x1), fpr(x1), fnr(x2),
+ * fpr(x2), the score at x1, x1, x2, status, then per point min_i (c_miss * fnr_i) * p + (c_fa * fpr_i) * (1 - p) (c_det; the
+ * caller divides by c_def).  x1 = first i with fnr_i - fpr_i >= 0, x2 = last i with fnr_i - fpr_i < 0.  Optional (NULL to
+ * skip): order_dev int32 [n] trial indices in sorted order, fnr_dev / fpr_dev fp64 [n] curves.  stage_events: NULL, or 11
+ * cudaEvent_t recorded on the stream before the keys pass, after it, after each of the 8 radix passes and after the
+ * evaluation (profiling).  Argument errors are refused before anything is launched; the host never waits on the device. */
+int ws_metrics_eval(const double* scores_dev, const unsigned char* labels_dev, long long n, const double* p_target,
+                    const double* c_miss, const double* c_fa, int n_points, void* work_dev, size_t work_bytes,
+                    double* out_dev, int* order_dev, double* fnr_dev, double* fpr_dev, void* stream,
+                    void* const* stage_events);
+
 #ifdef __cplusplus
 }
 #endif

@@ -119,6 +119,10 @@ _PROTOS = {
                                   C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "ws_diar_laplacian": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),
+    "ws_metrics_work_bytes": (C.c_size_t, [C.c_longlong]),
+    "ws_metrics_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                  C.POINTER(C.c_double), C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_PROTOS.keys())
 
