@@ -40,6 +40,8 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
  * returns an error on such an engine. */
 int ws_engine_create_plan_check(const char* model_name, const char* precision, int feat_dim, int embed_dim, ws_engine** out);
 /* options: "two_emb_layer", "emb_bn" (model_args), "cuda_graph" (default 1), "force_simt" (debug cross-check),
+ * "sample_rate" (8000 or 16000, default 16000: the rate of the waveforms the extract_wav entry points receive; their fbank
+ * writes feat_dim mel bins, 4 <= feat_dim <= 128; any other rate is refused - resample first, as the reference does),
  * "tc_version" (2: persistent / TMA-store tensor-core kernel, 3 (default): + weight-sharing CTA clusters on the large layers;
  * any other value is an error),
  * "res2_fused" (default 1: ECAPA Res2 chains run as one fused persistent kernel per stage for 16-bit precisions) */
@@ -116,8 +118,12 @@ long long ws_engine_last_launches(const ws_engine* e);
 void ws_engine_destroy(ws_engine* e);
 
 /* ---- fbank + CMN: replaces torchaudio.compliance.kaldi.fbank as called at processor.py:518-525 /
- *      cli/speaker.py:92-99 and Fbank::Compute (runtime/core/frontend/fbank.h:138-198). */
+ *      cli/speaker.py:92-99 and Fbank::Compute (runtime/core/frontend/fbank.h:138-198).  The entry points without a rate
+ *      are 16 kHz / 80 bins; the _at variants take sample_rate 8000 or 16000 (25 ms frames every 10 ms: 200 / 80 or
+ *      400 / 160 samples, a 256- or 512-point FFT) and 4 <= num_mel_bins <= 128, and refuse anything else before launching. */
 int ws_fbank_num_frames(int nsamples);
+/* frames of nsamples samples at sample_rate (0 below one frame); -1 for a rate other than 8000 / 16000 */
+int ws_fbank_num_frames_at(int nsamples, int sample_rate);
 /* Sinc resampling of (B, n_in) waveforms (int16 or float32) to new_freq: torchaudio.transforms.Resample(orig_freq, new_freq)
  * with its defaults, as the reference applies it before fbank (dataset/processor.py:242-262, cli/speaker.py:157-159).
  * out_dev: fp32 (B, out_ld), the first ws_resample_out_len(n_in, orig, new) = ceil(new * n_in / orig) samples of each row. */
@@ -126,12 +132,19 @@ int ws_resample(const void* wav_dev, int wav_is_i16, long long wav_ld, int n_in,
                 float* out_dev, long long out_ld, void* stream);
 int ws_fbank(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B, const char* window_type,
              int apply_cmn, float* feats_dev, void* stream);
+/* feats_dev fp32 [B][ws_fbank_num_frames_at(nsamples, sample_rate)][num_mel_bins]; a waveform shorter than one frame is refused */
+int ws_fbank_at(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B, const char* window_type,
+                int sample_rate, int num_mel_bins, int apply_cmn, float* feats_dev, void* stream);
 /* Ragged fbank, one launch: row b = n_frames_dev[b] frames starting at sample offsets_dev[b] of the flat buffer wav_dev
  * (total_samples samples); feats_dev fp32 [B][max_frames][80], rows behind n_frames_dev[b] are not written.  No CMN.  A frame
  * depends on its own 400 samples only, so a long segment may be presented as several rows (row k starting 160 * C * k samples
  * later) with identical results.  The caller guarantees offsets_dev[b] + 160 * (n_frames_dev[b] - 1) + 400 <= total_samples. */
 int ws_fbank_ragged(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
                     const int* n_frames_dev, int max_frames, int B, const char* window_type, float* feats_dev, void* stream);
+/* the same at sample_rate with num_mel_bins: feats_dev [B][max_frames][num_mel_bins], frames of the rate's geometry */
+int ws_fbank_ragged_at(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
+                       const int* n_frames_dev, int max_frames, int B, const char* window_type, int sample_rate, int num_mel_bins,
+                       float* feats_dev, void* stream);
 
 /* ---- generic fused conv operator (channels-last), the building block of the engine; exported for parity tests
  *      against torch conv1d/conv2d.  Replaces Conv1dReluBn (ecapa_tdnn.py:85-106), BasicBlock convs

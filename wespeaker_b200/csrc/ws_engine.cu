@@ -130,31 +130,43 @@ int run_plan(ws_engine* e, Plan* p, cudaStream_t s, int staged) {
     return 0;
 }
 
-const FbankTables* fbank_tables(ws_engine* e, const char* window_type) {
+// why the frontend cannot run at (sample_rate, bins) (nullptr = it can)
+const char* fbank_unsupported(int sample_rate, int bins) {
+    if (ws_fbank_frame_len(sample_rate) == 0) return "sample rate must be 8000 or 16000 (resample first)";
+    if (bins < 4 || bins > 128) return "num_mel_bins must be in [4, 128]";
+    return nullptr;
+}
+
+// Window and mel banks of one (window type, sample rate, bin count), uploaded on first use.  Restates torchaudio kaldi.py
+// _feature_window_function (25 ms, non-periodic) and get_mel_banks (20 Hz .. Nyquist, FFT bin width sample_rate / Nfft) in
+// float32 like the reference.
+const FbankTables* fbank_tables(ws_engine* e, const char* window_type, int rate, int nb) {
     const std::string wt = window_type ? window_type : "hamming";
-    auto it = e->fb.find(wt);
+    if (const char* why = fbank_unsupported(rate, nb)) { set_err(std::string("fbank: ") + why); return nullptr; }
+    const auto key = std::make_tuple(wt, rate, nb);
+    auto it = e->fb.find(key);
     if (it != e->fb.end()) return &it->second;
-    std::vector<float> win(400);
-    for (int j = 0; j < 400; ++j) {
-        const double c = std::cos(2.0 * M_PI * j / 399.0);
+    const int fl = ws_fbank_frame_len(rate), nfft = rate == 16000 ? 512 : 256, nbins_fft = nfft / 2;
+    std::vector<float> win(fl);
+    for (int j = 0; j < fl; ++j) {
+        const double c = std::cos(2.0 * M_PI * j / (fl - 1));
         if (wt == "hamming") win[j] = (float)(0.54 - 0.46 * c);
         else if (wt == "povey") win[j] = (float)std::pow(0.5 - 0.5 * c, 0.85);
         else if (wt == "hanning") win[j] = (float)(0.5 - 0.5 * c);
         else if (wt == "rectangular") win[j] = 1.f;
         else { set_err("unknown window_type " + wt); return nullptr; }
     }
-    // torchaudio kaldi.py get_mel_banks (80 bins, 20 Hz .. Nyquist, padded 512) in float32 like the reference
-    const int nb = 80, nfft = 256;
-    const double mel_low = 1127.0 * std::log(1.0 + 20.0 / 700.0), mel_high = 1127.0 * std::log(1.0 + 8000.0 / 700.0);
+    const double mel_low = 1127.0 * std::log(1.0 + 20.0 / 700.0), mel_high = 1127.0 * std::log(1.0 + 0.5 * rate / 700.0);
     const float delta = (float)((mel_high - mel_low) / (nb + 1)), lowf = (float)mel_low;
-    std::vector<std::vector<float>> rows(nb, std::vector<float>(nfft, 0.f));
+    const float bin_width = (float)rate / (float)nfft;
+    std::vector<std::vector<float>> rows(nb, std::vector<float>(nbins_fft, 0.f));
     std::vector<int> start(nb, 0), len(nb, 0);
     int maxlen = 1;
     for (int m = 0; m < nb; ++m) {
         const float left = lowf + (float)m * delta, center = lowf + ((float)m + 1.0f) * delta, right = lowf + ((float)m + 2.0f) * delta;
         int first = -1, last = -1;
-        for (int k = 0; k < nfft; ++k) {
-            const float mel = 1127.0f * std::log(1.0f + (31.25f * (float)k) / 700.0f);
+        for (int k = 0; k < nbins_fft; ++k) {
+            const float mel = 1127.0f * std::log(1.0f + (bin_width * (float)k) / 700.0f);
             const float up = (mel - left) / (center - left), down = (right - mel) / (right - center);
             const float wv = std::max(0.f, std::min(up, down));
             rows[m][k] = wv;
@@ -166,18 +178,17 @@ const FbankTables* fbank_tables(ws_engine* e, const char* window_type) {
     for (int m = 0; m < nb; ++m)
         for (int i = 0; i < len[m]; ++i) melw[(size_t)m * maxlen + i] = rows[m][start[m] + i];
     FbankTables t;
-    t.maxlen = maxlen;
-    if (cudaMalloc(&t.window, 400 * 4) != cudaSuccess || cudaMalloc(&t.melw, melw.size() * 4) != cudaSuccess ||
+    t.rate = rate; t.bins = nb; t.maxlen = maxlen;
+    if (cudaMalloc(&t.window, fl * 4) != cudaSuccess || cudaMalloc(&t.melw, melw.size() * 4) != cudaSuccess ||
         cudaMalloc(&t.melstart, nb * 4) != cudaSuccess || cudaMalloc(&t.mellen, nb * 4) != cudaSuccess) {
         set_err("fbank tables: cudaMalloc failed");
         return nullptr;
     }
-    cudaMemcpy(t.window, win.data(), 400 * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(t.window, win.data(), fl * 4, cudaMemcpyHostToDevice);
     cudaMemcpy(t.melw, melw.data(), melw.size() * 4, cudaMemcpyHostToDevice);
     cudaMemcpy(t.melstart, start.data(), nb * 4, cudaMemcpyHostToDevice);
     cudaMemcpy(t.mellen, len.data(), nb * 4, cudaMemcpyHostToDevice);
-    e->fb[wt] = t;
-    return &e->fb[wt];
+    return &(e->fb[key] = t);
 }
 
 // engine-less fbank tables for ws_fbank()
@@ -188,12 +199,13 @@ ws_engine* fbank_holder(int device) {
     return h;
 }
 
-// fbank (+ CMN) of B waveforms of nsamples samples (the longest, with lens) into feats [B][T][80]; offs / lens: ws_launch_fbank
+// fbank (+ CMN) of B waveforms of nsamples samples (the longest, with lens) into feats [B][T][t->bins]; offs / lens: ws_launch_fbank
 int fbank_into(const FbankTables* t, const void* wav, int is_i16, long long wav_ld, int nsamples, int B, int apply_cmn, float* feats,
                cudaStream_t s, const long long* offs = nullptr, const int* lens = nullptr) {
-    const int T = ws_fbank_num_frames(nsamples);
-    WS_CKS(ws_launch_fbank(wav, is_i16, wav_ld, nsamples, B, T, t->window, t->melw, t->melstart, t->mellen, t->maxlen, feats, s, offs, lens));
-    if (apply_cmn) WS_CKS(ws_launch_cmn(feats, B, T, 80, s, lens));
+    const int T = ws_fbank_num_frames_at(nsamples, t->rate);
+    WS_CKS(ws_launch_fbank(wav, is_i16, wav_ld, nsamples, B, T, t->rate, t->bins, t->window, t->melw, t->melstart, t->mellen, t->maxlen,
+                           feats, s, offs, lens));
+    if (apply_cmn) WS_CKS(ws_launch_cmn(feats, B, T, t->bins, s, lens));
     return 0;
 }
 
@@ -241,12 +253,13 @@ int begin_run(Run& r, int B, int T, bool masked, int samples = -1, const char* w
     ws_engine* e = r.e;
     if (const char* nr = not_runnable(e)) { set_err(std::string(r.who) + nr); return 1; }
     if (samples >= 0) {
-        if (e->feat_dim != 80) { set_err(std::string(r.who) + ": the fbank frontend produces 80 bins"); return 1; }
-        T = ws_fbank_num_frames(samples);
+        // the fbank frontend writes feat_dim mel bins at the engine's sample rate
+        if (const char* why = fbank_unsupported(e->sample_rate, e->feat_dim)) { set_err(std::string(r.who) + ": " + why); return 1; }
+        T = ws_fbank_num_frames_at(samples, e->sample_rate);
         if (T <= 0) { set_err(std::string(r.who) + ": waveforms shorter than one 25 ms frame"); return 1; }
     }
     if ((r.p = plan_of(e, B, T, masked)) == nullptr) return 1;
-    if (samples >= 0 && (r.fb = fbank_tables(e, window_type)) == nullptr) return 1;
+    if (samples >= 0 && (r.fb = fbank_tables(e, window_type, e->sample_rate, e->feat_dim)) == nullptr) return 1;
     r.s = r.host || !e->lanes[r.p->lane] ? e->st : e->lanes[r.p->lane];
     if (!r.host) {
         WS_CK(cudaEventRecord(e->ev_in, r.user));
@@ -345,6 +358,11 @@ int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
         }
         if (e->use_tc) e->use_tc = (int)value;
     }
+    else if (k == "sample_rate") {   // the waveform entry points' rate; plans do not depend on it, so they are kept
+        if (ws_fbank_frame_len((int)value) == 0 || value != (int)value) { set_err("sample_rate must be 8000 or 16000 (resample first)"); return 1; }
+        e->sample_rate = (int)value;
+        return 0;
+    }
     else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "plan_lanes" && k != "conv3x3_strided" && k != "astp_fused" && k != "plan_trace") { set_err("unknown option " + k); return 1; }
     e->opts[k] = value;
     e->plans.clear();
@@ -423,7 +441,8 @@ static int extract_wav_masked_impl(ws_engine* e, const void* wav_dev, int wav_is
     if (!e || !wav_dev || !n_samples_dev || !embs_dev || (ragged && !offsets_dev)) { set_err(std::string(who) + ": null argument"); return 1; }
     Run r{e, who, false, (cudaStream_t)stream};
     if (begin_run(r, B, 0, true, max_samples, window_type)) return 1;
-    WS_CKS(ws_launch_frames_from_samples(n_samples_dev, r.p->lens, B, r.p->T, r.s));
+    WS_CKS(ws_launch_frames_from_samples(n_samples_dev, r.p->lens, B, r.p->T, ws_fbank_frame_len(e->sample_rate),
+                                         ws_fbank_frame_shift(e->sample_rate), r.s));
     if (fbank_into(r.fb, wav_dev, wav_is_i16, wav_ld, max_samples, B, 1, r.p->feats_in, r.s, offsets_dev, r.p->lens)) return 1;
     return finish_run(r, 3, embs_dev, join);
 }
@@ -453,32 +472,62 @@ int ws_engine_forward_host(ws_engine* e, const float* feats_host, int B, int T, 
     return finish_run(r, 0, embs_host, true);
 }
 
-int ws_fbank_num_frames(int nsamples) { return nsamples < 400 ? 0 : 1 + (nsamples - 400) / 160; }
+int ws_fbank_num_frames(int nsamples) { return ws_fbank_num_frames_at(nsamples, 16000); }
+
+int ws_fbank_num_frames_at(int nsamples, int sample_rate) {
+    const int fl = ws_fbank_frame_len(sample_rate), sh = ws_fbank_frame_shift(sample_rate);
+    if (fl == 0) { set_err("ws_fbank_num_frames_at: sample rate must be 8000 or 16000"); return -1; }
+    return nsamples < fl ? 0 : 1 + (nsamples - fl) / sh;
+}
+
+// the tables of (window_type, sample_rate, bins) on the current device, for the engine-less fbank entry points
+static const FbankTables* device_fbank_tables(const char* window_type, int sample_rate, int bins) {
+    int dev = 0;
+    const cudaError_t ce = cudaGetDevice(&dev);
+    if (ce != cudaSuccess) { set_err(std::string("cudaGetDevice: ") + cudaGetErrorString(ce)); return nullptr; }
+    return fbank_tables(fbank_holder(dev), window_type, sample_rate, bins);
+}
 
 int ws_fbank(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B, const char* window_type,
              int apply_cmn, float* feats_dev, void* stream) {
     if (!wav_dev || !feats_dev) { set_err("ws_fbank: null argument"); return 1; }
-    int dev = 0;
-    WS_CK(cudaGetDevice(&dev));
-    const FbankTables* t = fbank_tables(fbank_holder(dev), window_type);
+    const FbankTables* t = device_fbank_tables(window_type, 16000, 80);
     if (!t) return 1;
     return fbank_into(t, wav_dev, wav_is_i16, wav_ld, nsamples, B, apply_cmn, feats_dev, (cudaStream_t)stream);
 }
 
-int ws_fbank_ragged(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
-                    const int* n_frames_dev, int max_frames, int B, const char* window_type, float* feats_dev, void* stream) {
+int ws_fbank_at(const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B, const char* window_type,
+                int sample_rate, int num_mel_bins, int apply_cmn, float* feats_dev, void* stream) {
+    if (!wav_dev || !feats_dev || B < 0) { set_err("ws_fbank_at: bad argument"); return 1; }
+    if (const char* why = fbank_unsupported(sample_rate, num_mel_bins)) { set_err(std::string("ws_fbank_at: ") + why); return 1; }
+    if (nsamples < ws_fbank_frame_len(sample_rate)) { set_err("ws_fbank_at: waveform shorter than one 25 ms frame"); return 1; }
+    const FbankTables* t = device_fbank_tables(window_type, sample_rate, num_mel_bins);
+    if (!t) return 1;
+    return fbank_into(t, wav_dev, wav_is_i16, wav_ld, nsamples, B, apply_cmn, feats_dev, (cudaStream_t)stream);
+}
+
+int ws_fbank_ragged_at(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
+                       const int* n_frames_dev, int max_frames, int B, const char* window_type, int sample_rate, int num_mel_bins,
+                       float* feats_dev, void* stream) {
     if (!wav_dev || !offsets_dev || !n_frames_dev || !feats_dev || B < 0 || max_frames < 0 || total_samples < 0) {
         set_err("ws_fbank_ragged: bad argument"); return 1;
     }
+    if (const char* why = fbank_unsupported(sample_rate, num_mel_bins)) { set_err(std::string("ws_fbank_ragged: ") + why); return 1; }
     if (B > 65535) { set_err("ws_fbank_ragged: more than 65535 rows in one launch"); return 1; }
-    int dev = 0;
-    WS_CK(cudaGetDevice(&dev));
-    const FbankTables* t = fbank_tables(fbank_holder(dev), window_type);
+    const FbankTables* t = device_fbank_tables(window_type, sample_rate, num_mel_bins);
     if (!t) return 1;
     // the launcher's size check is per row there; rows are placed by the caller here, which vouches for them
-    WS_CKS(ws_launch_fbank(wav_dev, wav_is_i16, 0, max_frames > 0 ? (max_frames - 1) * 160 + 400 : 0, B, max_frames, t->window,
-                           t->melw, t->melstart, t->mellen, t->maxlen, feats_dev, (cudaStream_t)stream, offsets_dev, n_frames_dev));
+    const int fl = ws_fbank_frame_len(sample_rate), sh = ws_fbank_frame_shift(sample_rate);
+    WS_CKS(ws_launch_fbank(wav_dev, wav_is_i16, 0, max_frames > 0 ? (max_frames - 1) * sh + fl : 0, B, max_frames, sample_rate,
+                           num_mel_bins, t->window, t->melw, t->melstart, t->mellen, t->maxlen, feats_dev, (cudaStream_t)stream,
+                           offsets_dev, n_frames_dev));
     return 0;
+}
+
+int ws_fbank_ragged(const void* wav_dev, int wav_is_i16, long long total_samples, const long long* offsets_dev,
+                    const int* n_frames_dev, int max_frames, int B, const char* window_type, float* feats_dev, void* stream) {
+    return ws_fbank_ragged_at(wav_dev, wav_is_i16, total_samples, offsets_dev, n_frames_dev, max_frames, B, window_type, 16000, 80,
+                              feats_dev, stream);
 }
 
 // ---- resampling (torchaudio.transforms.Resample defaults: sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99)
@@ -544,7 +593,7 @@ static int extract_wav_impl(ws_engine* e, const void* wav_dev, int wav_is_i16, l
     if (begin_run(r, B, 0, false, nsamples, window_type)) return 1;
     if (fbank_into(r.fb, wav_dev, wav_is_i16, wav_ld, nsamples, B, 1, r.p->feats_in, r.s)) return 1;
     if (feats_out_dev)
-        WS_CK(cudaMemcpyAsync(feats_out_dev, r.p->feats_in, (size_t)B * r.p->T * 80 * 4, cudaMemcpyDeviceToDevice, r.s));
+        WS_CK(cudaMemcpyAsync(feats_out_dev, r.p->feats_in, (size_t)B * r.p->T * e->feat_dim * 4, cudaMemcpyDeviceToDevice, r.s));
     return finish_run(r, 2, embs_dev, join);
 }
 int ws_engine_extract_wav(ws_engine* e, const void* wav_dev, int wav_is_i16, long long wav_ld, int nsamples, int B,

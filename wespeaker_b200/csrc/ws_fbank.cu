@@ -1,19 +1,28 @@
-// Kaldi-compatible 80-bin log-mel fbank + per-utterance CMN on the GPU (HBM-bound: 128 KB in, 63 KB out per
-// 2 s utterance).  Restates what the reference gets from torchaudio.compliance.kaldi.fbank with the arguments
-// of wespeaker/dataset/processor.py:518-525 / cli/speaker.py:92-97 (SURVEY.md Appendix B); native twin of
-// runtime/core/frontend/fbank.h:138-198.
+// Kaldi-compatible log-mel fbank + per-utterance CMN on the GPU (HBM-bound: 128 KB in, 63 KB out per 2 s utterance at
+// 16 kHz / 80 bins).  Restates what the reference gets from torchaudio.compliance.kaldi.fbank with the arguments of
+// wespeaker/dataset/processor.py:518-525 / cli/speaker.py:92-97 (SURVEY.md Appendix B); native twin of
+// runtime/core/frontend/fbank.h:138-198.  Two sample rates: 16 kHz (400-sample frames, 160-sample shift, 512-point FFT)
+// and 8 kHz (200 / 80 samples, 256-point FFT), the rates of the reference's recipes; 4..128 mel bins.
 //
-// One warp per 25 ms frame (8 frames per block): coalesced sample loads, DC removal via warp-shuffle sum,
-// pre-emphasis, window, then a 512-point real FFT computed as a 256-point complex radix-2 FFT in shared memory
-// (twiddles from sincospif, exact argument reduction) + the real-input split step, power spectrum, triangular mel
-// filters as short per-bin dot products (each lane owns bins lane, lane+32, lane+64), log with the float-eps floor.
+// One warp per 25 ms frame (8 frames per block): coalesced sample loads, DC removal via warp-shuffle sum, pre-emphasis,
+// window, then an Nfft-point real FFT computed as an Nfft/2-point complex FFT in registers and warp shuffles + the
+// real-input split step, power spectrum, triangular mel filters as short per-bin dot products (each lane owns bins lane,
+// lane+32, lane+64, lane+96), log with the float-eps floor.
 #include "ws_kernels.cuh"
-#include <cstdlib>
 
 namespace {
 
-constexpr int kFrameLen = 400, kFrameShift = 160, kNfft = 512, kBins = 80;
+constexpr int kMaxBins = 128;
 constexpr float kEps = 1.1920928955078125e-07f;
+
+// frame geometry of the Nfft-point transform: 25 ms frames and a 10 ms shift at Nfft * 31.25 Hz
+template <int NFFT> struct Geom {
+    static constexpr int kFrameLen = NFFT * 25 / 32;   // 400 | 200 samples
+    static constexpr int kShift = NFFT * 10 / 32;      // 160 | 80 samples
+    static constexpr int kN2 = NFFT / 2;               // complex FFT length
+    static constexpr int kR = kN2 / 32;                // complex values per lane
+    static constexpr int kPairSlots = (kFrameLen / 2 + 31) / 32;   // sample-pair registers per lane
+};
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -36,139 +45,50 @@ __device__ __forceinline__ float2 ld_sample2(const void* wav, int is_i16, long l
     return *reinterpret_cast<const float2*>((const float*)wav + i);
 }
 
-__global__ void __launch_bounds__(256) fbank_kernel(const void* __restrict__ wav, int is_i16, long long wav_ld, int T,
-                                                    const float* __restrict__ window, const float* __restrict__ melw,
-                                                    const int* __restrict__ melstart, const int* __restrict__ mellen,
-                                                    int mel_maxlen, float* __restrict__ feats) {
-    __shared__ float2 s_tw[256];        // W_512^k = exp(-2*pi*i*k/512)
-    __shared__ float2 s_z[8][256];      // per-warp FFT buffer
-    __shared__ float s_p[8][256];       // per-warp power spectrum (bins 0..255; Nyquist has zero mel weight)
-    __shared__ float s_win[kFrameLen];
-    __shared__ float s_melw[kBins * 20];
-    __shared__ short s_mels[kBins], s_mell[kBins];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    {
-        float sn, cs;
-        sincospif((float)threadIdx.x / 256.0f, &sn, &cs);
-        s_tw[threadIdx.x] = make_float2(cs, -sn);
-        for (int i = threadIdx.x; i < kFrameLen; i += 256) s_win[i] = window[i];
-        for (int i = threadIdx.x; i < kBins * mel_maxlen; i += 256) s_melw[(i / mel_maxlen) * 20 + (i % mel_maxlen)] = melw[i];
-        if (threadIdx.x < kBins) { s_mels[threadIdx.x] = (short)melstart[threadIdx.x]; s_mell[threadIdx.x] = (short)mellen[threadIdx.x]; }
-    }
-    __syncthreads();
-    const int b = blockIdx.y;
-    const int frame = blockIdx.x * 8 + warp;
-    if (frame >= T) return;
-    // frame starts are multiples of 160 samples, so pair loads are aligned whenever b * wav_ld is even (else scalar loads)
-    const long long base = (long long)b * wav_ld + (long long)frame * kFrameShift;
-
-    // each lane owns sample pairs n = lane + 32k (k < 7, n < 200): ONE pass over the samples (coalesced pair loads)
-    float2 x[7];
-    float s = 0.f;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) {
-        const int n = lane + 32 * k;
-        x[k] = n < kFrameLen / 2 ? ld_sample2(wav, is_i16, base + 2 * n) : make_float2(0.f, 0.f);
-        s += x[k].x + x[k].y;
-    }
-    const float mu = warp_sum(s) / (float)kFrameLen;   // remove_dc_offset
-
-    // z[n] = y[2n] + i*y[2n+1], y = window * ((x - mu) - 0.97 * (x_prev - mu)); x[2n-1] comes from the neighbouring lane
-    float2* z = s_z[warp];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        const int n = lane + 32 * k;
-        float2 v = make_float2(0.f, 0.f);
-        if (k < 7) {
-            // previous odd sample: lane-1 of the same k, or lane 31 of k-1 for lane 0 (replicate-pad at n = 0)
-            float prev_same = __shfl_up_sync(0xffffffffu, x[k].y, 1);
-            float prev_wrap = __shfl_sync(0xffffffffu, k > 0 ? x[k > 0 ? k - 1 : 0].y : 0.f, 31);
-            if (n < kFrameLen / 2) {
-                const float xm1 = (lane > 0 ? prev_same : (k > 0 ? prev_wrap : x[0].x)) - mu;
-                const float x0 = x[k].x - mu, x1 = x[k].y - mu;
-                v.x = (x0 - 0.97f * xm1) * s_win[2 * n];
-                v.y = (x1 - 0.97f * x0) * s_win[2 * n + 1];
-            }
-        }
-        z[__brev((unsigned)n) >> 24] = v;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int st = 1; st <= 8; ++st) {
-        const int half = 1 << (st - 1);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int idx = lane + 32 * k;
-            const int j = idx & (half - 1);
-            const int i0 = ((idx >> (st - 1)) << st) + j;
-            const int i1 = i0 + half;
-            const float2 w = s_tw[j << (9 - st)];
-            const float2 u = z[i0], a = z[i1];
-            const float2 v = make_float2(a.x * w.x - a.y * w.y, a.x * w.y + a.y * w.x);
-            z[i0] = make_float2(u.x + v.x, u.y + v.y);
-            z[i1] = make_float2(u.x - v.x, u.y - v.y);
-        }
-        __syncwarp();
-    }
-    // split step: X[k] = E[k] + W_512^k * O[k],  E = (Z[k] + conj(Z[256-k]))/2,  O = -i (Z[k] - conj(Z[256-k]))/2
-    float* pw = s_p[warp];
-#pragma unroll
-    for (int k8 = 0; k8 < 8; ++k8) {
-        const int k = lane + 32 * k8;
-        const float2 a = z[k];
-        const float2 c = z[(256 - k) & 255];
-        const float er = 0.5f * (a.x + c.x), ei = 0.5f * (a.y - c.y);
-        const float orr = 0.5f * (a.y + c.y), oi = -0.5f * (a.x - c.x);
-        const float2 w = s_tw[k];
-        const float xr = er + (orr * w.x - oi * w.y);
-        const float xi = ei + (orr * w.y + oi * w.x);
-        pw[k] = xr * xr + xi * xi;
-    }
-    __syncwarp();
-    float* out = feats + ((long long)b * T + frame) * kBins;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int m = lane + 32 * k;
-        if (m < kBins) {
-            const int st = s_mels[m], len = s_mell[m];
-            const float* w = s_melw + m * 20;
-            float e = 0.f;
-            for (int i = 0; i < len; ++i) e = fmaf(pw[st + i], w[i], e);
-            out[m] = logf(fmaxf(e, kEps));
-        }
-    }
-}
-
-// ---- version 2: the 256-point complex FFT never touches shared memory.  Lane L holds z[L + 32k] (k < 8), so
-//   X[f1 + 8 f0] = sum_L W32^(L f0) * ( W256^(L f1) * sum_k z[L + 32k] W8^(k f1) )
-// = an 8-point DFT in each lane's registers, one twiddle per register, and a 32-point DIF across the lanes done with
+// The N2 = Nfft/2-point complex FFT never touches shared memory.  With R = N2/32, lane L holds z[L + 32k] (k < R), so
+//   X[f1 + R f0] = sum_L W32^(L f0) * ( W_N2^(L f1) * sum_k z[L + 32k] W_R^(k f1) )
+// = an R-point DFT in each lane's registers, one twiddle per register, and a 32-point DIF across the lanes done with
 // __shfl_xor butterflies (distance 16, 8, 4, 2, 1; result for f0 = bitrev5(L)).  The spectrum goes to smem once for the
-// real-input split step (which pairs bin k with bin 256-k).  8 dependent smem passes + __syncwarp()s become 40 shuffle
-// steps with 16 independent values each.
+// real-input split step (which pairs bin k with bin N2-k).
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ int zpad(int f) { return f + (f >> 3); }   // skewed smem index of spectrum bin f
+// register i of the R-point DIF holds frequency bitrev_log2(R)(i)
+template <int R> __device__ __forceinline__ int reg_freq(int i) {
+    return R == 8 ? (((i & 1) << 2) | (i & 2) | ((i & 4) >> 2)) : (((i & 1) << 1) | ((i & 2) >> 1));
+}
 
-__global__ void __launch_bounds__(256) fbank_kernel2(const void* __restrict__ wav, int is_i16, long long wav_ld, int T,
-                                                     const float* __restrict__ window, const float* __restrict__ melw,
-                                                     const int* __restrict__ melstart, const int* __restrict__ mellen,
-                                                     int mel_maxlen, float* __restrict__ feats,
-                                                     const long long* __restrict__ offs, const int* __restrict__ lens) {
-    __shared__ float2 s_tw[256];        // W_512^k = exp(-2*pi*i*k/512)
-    __shared__ float2 s_z[8][288];      // per-warp spectrum, index zpad(f)
-    __shared__ float s_p[8][256];       // per-warp power spectrum (bins 0..255; Nyquist has zero mel weight)
-    __shared__ float s_win[kFrameLen];
-    __shared__ float s_melw[kBins * 20];
-    __shared__ short s_mels[kBins], s_mell[kBins];
+// melw: [nbins][mel_maxlen] filter taps, staged in dynamic shared memory in rows of 4 * mel_ld4(mel_maxlen) floats.  Lanes
+// read the rows of consecutive bins in lockstep: 16-byte aligned rows allow 128-bit loads, and a row length of 4 mod 8
+// floats puts the 8 lanes of each 128-bit load phase in distinct banks.
+__host__ __device__ constexpr int mel_ld4(int mel_maxlen) { return ((mel_maxlen + 3) / 4) | 1; }
+// NG = ceil(nbins / 32): the mel bins each lane owns
+template <int NFFT, int NG>
+__global__ void __launch_bounds__(256) fbank_kernel(const void* __restrict__ wav, int is_i16, long long wav_ld, int T,
+                                                    const float* __restrict__ window, const float* __restrict__ melw,
+                                                    const int* __restrict__ melstart, const int* __restrict__ mellen,
+                                                    int nbins, int mel_maxlen, float* __restrict__ feats,
+                                                    const long long* __restrict__ offs, const int* __restrict__ lens) {
+    using G = Geom<NFFT>;
+    constexpr int N2 = G::kN2, R = G::kR, FL = G::kFrameLen;
+    static_assert(R == 8 || R == 4, "fbank: 256- or 512-point FFT");
+    __shared__ float2 s_tw[N2];                 // W_Nfft^k = exp(-2*pi*i*k/Nfft)
+    __shared__ float2 s_z[8][N2 + N2 / 8];      // per-warp spectrum, index zpad(f)
+    __shared__ float s_p[8][N2];                // per-warp power spectrum (bins 0..N2-1; Nyquist has zero mel weight)
+    __shared__ float s_win[FL];
+    __shared__ short s_mels[kMaxBins], s_mell[kMaxBins];
+    extern __shared__ __align__(16) float s_melw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     {
-        float sn, cs;
-        sincospif((float)threadIdx.x / 256.0f, &sn, &cs);
-        s_tw[threadIdx.x] = make_float2(cs, -sn);
-        for (int i = threadIdx.x; i < kFrameLen; i += 256) s_win[i] = window[i];
-        for (int i = threadIdx.x; i < kBins * mel_maxlen; i += 256) s_melw[(i / mel_maxlen) * 20 + (i % mel_maxlen)] = melw[i];
-        if (threadIdx.x < kBins) { s_mels[threadIdx.x] = (short)melstart[threadIdx.x]; s_mell[threadIdx.x] = (short)mellen[threadIdx.x]; }
+        if (threadIdx.x < N2) {
+            float sn, cs;
+            sincospif((float)threadIdx.x / (float)N2, &sn, &cs);
+            s_tw[threadIdx.x] = make_float2(cs, -sn);
+        }
+        for (int i = threadIdx.x; i < FL; i += 256) s_win[i] = window[i];
+        for (int i = threadIdx.x; i < nbins * mel_maxlen; i += 256) s_melw[(i / mel_maxlen) * 4 * mel_ld4(mel_maxlen) + i % mel_maxlen] = melw[i];
+        if (threadIdx.x < nbins) { s_mels[threadIdx.x] = (short)melstart[threadIdx.x]; s_mell[threadIdx.x] = (short)mellen[threadIdx.x]; }
     }
     __syncthreads();
     const int b = blockIdx.y;
@@ -177,28 +97,31 @@ __global__ void __launch_bounds__(256) fbank_kernel2(const void* __restrict__ wa
     // ragged / length-masked input: utterance b starts at offs[b] (else b * wav_ld) and has lens[b] frames; frames behind
     // the end are neither read nor written (cmn_kernel zeroes them), so a ragged buffer is never read past its last sample
     if (lens != nullptr && frame >= lens[b]) return;
-    const long long base = (offs != nullptr ? offs[b] : (long long)b * wav_ld) + (long long)frame * kFrameShift;
+    // frame starts are multiples of the (even) shift, so pair loads are aligned whenever the row start is even
+    const long long base = (offs != nullptr ? offs[b] : (long long)b * wav_ld) + (long long)frame * G::kShift;
 
-    float2 x[7];
+    // each lane owns sample pairs n = lane + 32k (n < FL/2): ONE pass over the samples (coalesced pair loads)
+    float2 x[G::kPairSlots];
     float s = 0.f;
 #pragma unroll
-    for (int k = 0; k < 7; ++k) {
+    for (int k = 0; k < G::kPairSlots; ++k) {
         const int n = lane + 32 * k;
-        x[k] = n < kFrameLen / 2 ? ld_sample2(wav, is_i16, base + 2 * n) : make_float2(0.f, 0.f);
+        x[k] = n < FL / 2 ? ld_sample2(wav, is_i16, base + 2 * n) : make_float2(0.f, 0.f);
         s += x[k].x + x[k].y;
     }
-    const float mu = warp_sum(s) / (float)kFrameLen;   // remove_dc_offset
+    const float mu = warp_sum(s) / (float)FL;   // remove_dc_offset
 
-    // a[k] = z[lane + 32k] = y[2n] + i*y[2n+1], y = window * ((x - mu) - 0.97 * (x_prev - mu))
-    float2 a[8];
+    // a[k] = z[lane + 32k] = y[2n] + i*y[2n+1], y = window * ((x - mu) - 0.97 * (x_prev - mu)); x[2n-1] comes from the
+    // neighbouring lane (lane-1 of the same k, or lane 31 of k-1 for lane 0; replicate-pad at n = 0)
+    float2 a[R];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
+    for (int k = 0; k < R; ++k) {
         const int n = lane + 32 * k;
         float2 v = make_float2(0.f, 0.f);
-        if (k < 7) {
+        if (k < G::kPairSlots) {
             float prev_same = __shfl_up_sync(0xffffffffu, x[k].y, 1);
             float prev_wrap = __shfl_sync(0xffffffffu, k > 0 ? x[k > 0 ? k - 1 : 0].y : 0.f, 31);
-            if (n < kFrameLen / 2) {
+            if (n < FL / 2) {
                 const float xm1 = (lane > 0 ? prev_same : (k > 0 ? prev_wrap : x[0].x)) - mu;
                 const float x0 = x[k].x - mu, x1 = x[k].y - mu;
                 v.x = (x0 - 0.97f * xm1) * s_win[2 * n];
@@ -207,34 +130,34 @@ __global__ void __launch_bounds__(256) fbank_kernel2(const void* __restrict__ wa
         }
         a[k] = v;
     }
-    // ---- 8-point DIF over k in registers; afterwards register i holds f1 = bitrev3(i)
+    // ---- R-point DIF over k in registers; afterwards register i holds f1 = reg_freq<R>(i)
     {
         const float h = 0.70710678118654752440f;
         float2 t;
-        // stage 1: (k, k+4), twiddles W8^k
-        t = csub(a[0], a[4]); a[0] = cadd(a[0], a[4]); a[4] = t;
-        t = csub(a[1], a[5]); a[1] = cadd(a[1], a[5]); a[5] = make_float2(h * (t.x + t.y), h * (t.y - t.x));
-        t = csub(a[2], a[6]); a[2] = cadd(a[2], a[6]); a[6] = make_float2(t.y, -t.x);
-        t = csub(a[3], a[7]); a[3] = cadd(a[3], a[7]); a[7] = make_float2(h * (t.y - t.x), -h * (t.x + t.y));
-        // stage 2: (k, k+2) inside each half, twiddles 1, -i
+        if constexpr (R == 8) {
+            // stage 1 of 8: (k, k+4), twiddles W8^k
+            t = csub(a[0], a[4]); a[0] = cadd(a[0], a[4]); a[4] = t;
+            t = csub(a[1], a[5]); a[1] = cadd(a[1], a[5]); a[5] = make_float2(h * (t.x + t.y), h * (t.y - t.x));
+            t = csub(a[2], a[6]); a[2] = cadd(a[2], a[6]); a[6] = make_float2(t.y, -t.x);
+            t = csub(a[3], a[7]); a[3] = cadd(a[3], a[7]); a[7] = make_float2(h * (t.y - t.x), -h * (t.x + t.y));
+        }
+        // 4-point DIF on each group of 4 - (k, k+2), twiddles 1, -i; then neighbours
 #pragma unroll
-        for (int hb = 0; hb < 8; hb += 4) {
+        for (int hb = 0; hb < R; hb += 4) {
             t = csub(a[hb], a[hb + 2]); a[hb] = cadd(a[hb], a[hb + 2]); a[hb + 2] = t;
             t = csub(a[hb + 1], a[hb + 3]); a[hb + 1] = cadd(a[hb + 1], a[hb + 3]); a[hb + 3] = make_float2(t.y, -t.x);
         }
-        // stage 3: neighbours
 #pragma unroll
-        for (int hb = 0; hb < 8; hb += 2) {
+        for (int hb = 0; hb < R; hb += 2) {
             t = csub(a[hb], a[hb + 1]); a[hb] = cadd(a[hb], a[hb + 1]); a[hb + 1] = t;
         }
     }
-    // ---- twiddle W256^(lane * f1) = W512^(2 * lane * f1)
+    // ---- twiddle W_N2^(lane * f1) = W_Nfft^(2 * lane * f1)  (2 * 31 * (R-1) < Nfft: at most one half-turn to fold)
 #pragma unroll
-    for (int i = 1; i < 8; ++i) {
-        const int f1 = ((i & 1) << 2) | (i & 2) | ((i & 4) >> 2);
-        const int idx = 2 * lane * f1;
-        float2 w = s_tw[idx & 255];
-        if (idx >= 256) w = make_float2(-w.x, -w.y);
+    for (int i = 1; i < R; ++i) {
+        const int idx = 2 * lane * reg_freq<R>(i);
+        float2 w = s_tw[idx & (N2 - 1)];
+        if (idx >= N2) w = make_float2(-w.x, -w.y);
         a[i] = cmul(a[i], w);
     }
     // ---- 32-point DIF across the lanes
@@ -242,33 +165,30 @@ __global__ void __launch_bounds__(256) fbank_kernel2(const void* __restrict__ wa
     for (int d = 16; d >= 1; d >>= 1) {
         const bool upper = (lane & d) == 0;
         const float sg = upper ? 1.f : -1.f;
-        const float2 w = upper ? make_float2(1.f, 0.f) : s_tw[(lane & (d - 1)) * (256 / d)];
+        const float2 w = upper ? make_float2(1.f, 0.f) : s_tw[(lane & (d - 1)) * (N2 / d)];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
+        for (int i = 0; i < R; ++i) {
             const float ox = __shfl_xor_sync(0xffffffffu, a[i].x, d);
             const float oy = __shfl_xor_sync(0xffffffffu, a[i].y, d);
             const float2 t = make_float2(fmaf(sg, a[i].x, ox), fmaf(sg, a[i].y, oy));   // upper: a + o, lower: o - a
             a[i] = cmul(t, w);
         }
     }
-    // lane L, register i holds Z[bitrev3(i) + 8 * bitrev5(L)]
+    // lane L, register i holds Z[reg_freq(i) + R * bitrev5(L)]
     float2* z = s_z[warp];
     {
         const int f0 = (int)(__brev((unsigned)lane) >> 27);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const int f1 = ((i & 1) << 2) | (i & 2) | ((i & 4) >> 2);
-            z[zpad(f1 + 8 * f0)] = a[i];
-        }
+        for (int i = 0; i < R; ++i) z[zpad(reg_freq<R>(i) + R * f0)] = a[i];
     }
     __syncwarp();
-    // split step: X[k] = E[k] + W_512^k * O[k],  E = (Z[k] + conj(Z[256-k]))/2,  O = -i (Z[k] - conj(Z[256-k]))/2
+    // split step: X[k] = E[k] + W_Nfft^k * O[k],  E = (Z[k] + conj(Z[N2-k]))/2,  O = -i (Z[k] - conj(Z[N2-k]))/2
     float* pw = s_p[warp];
 #pragma unroll
-    for (int k8 = 0; k8 < 8; ++k8) {
+    for (int k8 = 0; k8 < R; ++k8) {
         const int k = lane + 32 * k8;
         const float2 za = z[zpad(k)];
-        const float2 c = z[zpad((256 - k) & 255)];
+        const float2 c = z[zpad((N2 - k) & (N2 - 1))];
         const float er = 0.5f * (za.x + c.x), ei = 0.5f * (za.y - c.y);
         const float orr = 0.5f * (za.y + c.y), oi = -0.5f * (za.x - c.x);
         const float2 w = s_tw[k];
@@ -277,13 +197,13 @@ __global__ void __launch_bounds__(256) fbank_kernel2(const void* __restrict__ wa
         pw[k] = xr * xr + xi * xi;
     }
     __syncwarp();
-    float* out = feats + ((long long)b * T + frame) * kBins;
+    float* out = feats + ((long long)b * T + frame) * nbins;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
+    for (int k = 0; k < NG; ++k) {
         const int m = lane + 32 * k;
-        if (m < kBins) {
+        if (m < nbins) {
             const int st = s_mels[m], len = s_mell[m];
-            const float* w = s_melw + m * 20;
+            const float* w = s_melw + 4 * (m * mel_ld4(mel_maxlen));
             float e = 0.f;
             for (int i = 0; i < len; ++i) e = fmaf(pw[st + i], w[i], e);
             out[m] = logf(fmaxf(e, kEps));
@@ -315,19 +235,35 @@ __global__ void __launch_bounds__(256) cmn_kernel(float* __restrict__ feats, int
     }
 }
 
+template <int NFFT>
+cudaError_t launch_fbank(const void* wav, int is_i16, long long wav_ld, int B, int T, const float* window, const float* melw,
+                         const int* melstart, const int* mellen, int nbins, int mel_maxlen, float* feats, cudaStream_t s,
+                         const long long* offs, const int* lens) {
+    dim3 grid((T + 7) / 8, B);
+    const size_t smem = (size_t)nbins * 4 * mel_ld4(mel_maxlen) * sizeof(float);
+    auto kern = nbins <= 32 ? fbank_kernel<NFFT, 1> : nbins <= 64 ? fbank_kernel<NFFT, 2>
+              : nbins <= 96 ? fbank_kernel<NFFT, 3> : fbank_kernel<NFFT, 4>;
+    kern<<<grid, 256, smem, s>>>(wav, is_i16, wav_ld, T, window, melw, melstart, mellen, nbins, mel_maxlen, feats, offs, lens);
+    return cudaGetLastError();
+}
+
 }  // namespace
 
-const char* ws_launch_fbank(const void* wav, int wav_is_i16, long long wav_ld, int nsamples, int B, int T,
-                            const float* window400, const float* melw, const int* melstart, const int* mellen,
+int ws_fbank_frame_len(int sample_rate) { return sample_rate == 16000 ? 400 : sample_rate == 8000 ? 200 : 0; }
+int ws_fbank_frame_shift(int sample_rate) { return sample_rate == 16000 ? 160 : sample_rate == 8000 ? 80 : 0; }
+
+const char* ws_launch_fbank(const void* wav, int wav_is_i16, long long wav_ld, int nsamples, int B, int T, int sample_rate,
+                            int nbins, const float* window, const float* melw, const int* melstart, const int* mellen,
                             int mel_maxlen, float* feats, cudaStream_t s, const long long* offs, const int* lens) {
+    const int fl = ws_fbank_frame_len(sample_rate), sh = ws_fbank_frame_shift(sample_rate);
+    if (fl == 0) return "fbank: sample rate must be 8000 or 16000";
+    if (nbins < 4 || nbins > kMaxBins) return "fbank: mel bin count outside [4, 128]";
     if (T <= 0 || B <= 0) return nullptr;
-    if ((long long)(T - 1) * kFrameShift + kFrameLen > nsamples) return "fbank: T frames do not fit in nsamples";
-    if (mel_maxlen > 20) return "fbank: mel filter wider than the shared-memory table";
-    dim3 grid((T + 7) / 8, B);
-    static const bool v1 = getenv("WS_FBANK_V1") != nullptr;   // A/B knob: the shared-memory radix-2 version
-    if (v1 && !offs && !lens) fbank_kernel<<<grid, 256, 0, s>>>(wav, wav_is_i16, wav_ld, T, window400, melw, melstart, mellen, mel_maxlen, feats);
-    else fbank_kernel2<<<grid, 256, 0, s>>>(wav, wav_is_i16, wav_ld, T, window400, melw, melstart, mellen, mel_maxlen, feats, offs, lens);
-    cudaError_t e = cudaGetLastError();
+    if ((long long)(T - 1) * sh + fl > nsamples) return "fbank: T frames do not fit in nsamples";
+    if ((size_t)nbins * 4 * mel_ld4(mel_maxlen) * sizeof(float) > kFbankMaxMelBytes) return "fbank: mel filter table larger than the shared-memory limit";
+    const cudaError_t e = sample_rate == 16000
+        ? launch_fbank<512>(wav, wav_is_i16, wav_ld, B, T, window, melw, melstart, mellen, nbins, mel_maxlen, feats, s, offs, lens)
+        : launch_fbank<256>(wav, wav_is_i16, wav_ld, B, T, window, melw, melstart, mellen, nbins, mel_maxlen, feats, s, offs, lens);
     return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 

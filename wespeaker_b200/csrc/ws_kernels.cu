@@ -874,11 +874,12 @@ __global__ void lens_derive_kernel(int* __restrict__ lens, int B, int T, int lev
     lens[b] = l;
     for (int k = 1; k < levels; ++k) { l = (l - 1) / 2 + 1; lens[k * B + b] = l; }
 }
-// frames of an utterance of n samples (snip_edges, 25 ms / 10 ms at 16 kHz)
+// frames of an utterance of n samples (snip_edges, frames of frame_len samples every shift samples)
 // (clamped to [1, Tmax]: an utterance shorter than one frame is the caller's error, the reference's fbank fails on it too)
-__global__ void frames_from_samples_kernel(const int* __restrict__ nsamp, int* __restrict__ lens, int B, int Tmax) {
+__global__ void frames_from_samples_kernel(const int* __restrict__ nsamp, int* __restrict__ lens, int B, int Tmax, int frame_len,
+                                           int shift) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < B) lens[b] = max(1, min(Tmax, nsamp[b] < 400 ? 0 : 1 + (nsamp[b] - 400) / 160));
+    if (b < B) lens[b] = max(1, min(Tmax, nsamp[b] < frame_len ? 0 : 1 + (nsamp[b] - frame_len) / shift));
 }
 
 inline const char* last_err() {
@@ -991,8 +992,8 @@ const char* ws_launch_lens_derive(int* lens, int B, int T, int levels, cudaStrea
     lens_derive_kernel<<<(B + 127) / 128, 128, 0, s>>>(lens, B, T, levels);
     return last_err();
 }
-const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, cudaStream_t s) {
-    frames_from_samples_kernel<<<(B + 127) / 128, 128, 0, s>>>(nsamp, lens, B, Tmax);
+const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, int frame_len, int shift, cudaStream_t s) {
+    frames_from_samples_kernel<<<(B + 127) / 128, 128, 0, s>>>(nsamp, lens, B, Tmax, frame_len, shift);
     return last_err();
 }
 

@@ -17,7 +17,7 @@ const char* ws_launch_tstats(const void* x, int dt, int B, int F, int T, int C, 
 const char* ws_launch_zero_tail(void* x, float* lo, int dt, int B, int F, int T, int C, long long ld, const int* lens,
                                 cudaStream_t s);
 const char* ws_launch_lens_derive(int* lens, int B, int T, int levels, cudaStream_t s);
-const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, cudaStream_t s);
+const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, int frame_len, int shift, cudaStream_t s);
 // out[r][o] = act( sum_i W[o][i] * (in[r][i] + in2[r / rows_per_b][i]) + bias[o] ),  fp32 in/out, W fp32 [O][I]
 bool ws_linear_rows_big(long long in_ld, const float* in2, long long in2_ld, int R, int I, int O);
 const char* ws_launch_linear_rows(const float* in, long long in_ld, const float* in2, long long in2_ld,
@@ -72,9 +72,15 @@ const char* ws_launch_cam_gate(const void* x, int dt, int B, int T, int C, long 
                                cudaStream_t s);
 
 // ---- fbank + CMN (ws_fbank.cu)
-// wav: [B][wav_ld] samples in int16 range (float32 if wav_is_i16 == 0 else int16).  feats fp32 [B][T][80].
-const char* ws_launch_fbank(const void* wav, int wav_is_i16, long long wav_ld, int nsamples, int B, int T,
-                            const float* window400, const float* melw, const int* melstart, const int* mellen,
+// 25 ms frame length / 10 ms shift in samples at sample_rate 8000 or 16000 (0 for any other rate)
+int ws_fbank_frame_len(int sample_rate);
+int ws_fbank_frame_shift(int sample_rate);
+// the largest mel filter table (nbins rows of mel_maxlen taps, padded to 4 mod 8 floats) ws_launch_fbank stages in shared memory
+constexpr size_t kFbankMaxMelBytes = 16384;
+// wav: [B][wav_ld] samples in int16 range (float32 if wav_is_i16 == 0 else int16).  feats fp32 [B][T][nbins], 4 <= nbins <= 128;
+// window: ws_fbank_frame_len(sample_rate) taps; melw [nbins][mel_maxlen] taps of the filter that starts at FFT bin melstart[m]
+const char* ws_launch_fbank(const void* wav, int wav_is_i16, long long wav_ld, int nsamples, int B, int T, int sample_rate,
+                            int nbins, const float* window, const float* melw, const int* melstart, const int* mellen,
                             int mel_maxlen, float* feats, cudaStream_t s, const long long* offs = nullptr,
                             const int* lens = nullptr);   // offs: utterance b starts at wav + offs[b]; lens: frames per utterance
 const char* ws_launch_cmn(float* feats, int B, int T, int Fdim, cudaStream_t s, const int* lens = nullptr);

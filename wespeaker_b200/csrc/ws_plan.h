@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstring>
 #include <memory>
+#include <tuple>
 
 #include "../../include/wespeaker_b200.h"
 #include "ws_host.h"
@@ -23,7 +24,9 @@ struct HostT {
     }
 };
 
+// the fbank frontend's device tables for one (window type, sample rate, mel bin count)
 struct FbankTables {
+    int rate = 16000, bins = 80;
     float* window = nullptr;
     float* melw = nullptr;
     int* melstart = nullptr;
@@ -104,7 +107,8 @@ struct ws_engine {
     cudaStream_t lanes[kLanes] = {nullptr, nullptr, nullptr, nullptr};
     int next_lane = 0;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-    std::map<std::string, ws::FbankTables> fb;
+    std::map<std::tuple<std::string, int, int>, ws::FbankTables> fb;   // key: (window type, sample rate, mel bins)
+    int sample_rate = 16000;   // waveform entry points (option "sample_rate"); the mel bin count is feat_dim
     void* wav_dev = nullptr;
     size_t wav_bytes = 0;
     // double-buffered host->device pipeline (ws_engine_submit_wav_host / ws_engine_collect)

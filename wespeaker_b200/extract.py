@@ -13,8 +13,8 @@ tiled) — that is what makes batches rectangular there.  What changes is where 
 DataLoader worker processes on the CPU and ships features to the GPU (`extract.py:99-134`); here a pool of reader threads
 only decodes PCM, batches go through ``B200SpeakerModel.extract_stream`` (pinned int16 H2D of batch i+1 overlapping fbank +
 CMN + forward of batch i on the device), and whole utterances of equal length are batched together.
-Audio at another sample rate is resampled to ``resample_rate`` on the device (``frontend.resample`` = torchaudio's sinc
-resampler, `processor.py:242-262`).  The augmentation pipeline (``reverb_data`` / ``noise_data`` / ``aug_prob``),
+Audio at another sample rate is resampled to ``resample_rate`` (16000, or 8000 as in the SRE recipes) on the device
+(``frontend.resample`` = torchaudio's sinc resampler, `processor.py:242-262`).  The augmentation pipeline (``reverb_data`` / ``noise_data`` / ``aug_prob``),
 ``speed_perturb`` and SSL frontends are training-side features outside SURVEY.md section 8: requesting them raises.
 """
 from __future__ import annotations
@@ -79,6 +79,26 @@ def get_random_chunk(data: np.ndarray, chunk_len: int, rng: random.Random) -> np
     return np.tile(data, rep if data.ndim == 1 else (rep, 1))[:chunk_len]
 
 
+def frontend_args(test_conf: dict, feat_dim: int):
+    """(resample_rate, num_mel_bins) of the ``dataset_args`` the fused wav path computes: fbank at 8 or 16 kHz, 25 ms frames
+    every 10 ms, ``fbank_args.num_mel_bins`` equal to the model's feat_dim (the reference would fail in the forward pass on
+    any other count)."""
+    resample_rate = int(test_conf.get("resample_rate", 16000))
+    if resample_rate not in frontend.SAMPLE_RATES:
+        raise NotImplementedError(f"dataset_args.resample_rate {resample_rate}: the fbank kernel runs at "
+                                  f"{frontend.SAMPLE_RATES} Hz")
+    fb = test_conf.get("fbank_args", {}) or {}
+    if (float(fb.get("frame_length", 25)), float(fb.get("frame_shift", 10))) != (25.0, 10.0):
+        raise NotImplementedError("fbank_args frame_length / frame_shift other than 25 ms / 10 ms are outside the engine's "
+                                  "hot path")
+    num_mel_bins = int(fb.get("num_mel_bins", feat_dim))
+    if num_mel_bins != feat_dim:
+        raise ValueError(f"dataset_args.fbank_args.num_mel_bins = {num_mel_bins} does not match the model's feat_dim = "
+                         f"{feat_dim}")
+    frontend.check_rate_bins(resample_rate, num_mel_bins)
+    return resample_rate, num_mel_bins
+
+
 def _iter_raw(data_list):
     with open(data_list) as f:
         for line in f:
@@ -121,13 +141,8 @@ def extract(config="conf/config.yaml", **kwargs):
         raise NotImplementedError("only the fbank frontend is on the engine's hot path")
     if (configs.get("reverb_data") or configs.get("noise_data")) and float(configs.get("aug_prob", 0.0)) > 0.0:
         raise NotImplementedError("reverb / noise augmentation at extraction time is outside the engine's hot path")
-    resample_rate = int(test_conf.get("resample_rate", 16000))
-    if resample_rate != 16000:
-        raise NotImplementedError("the fbank kernel is built for 16 kHz (dataset_args.resample_rate)")
-    fb = test_conf.get("fbank_args", {})
-    if (int(fb.get("num_mel_bins", 80)), int(fb.get("frame_length", 25)), int(fb.get("frame_shift", 10))) != (80, 25, 10):
-        raise NotImplementedError("fbank_args other than 80 bins / 25 ms / 10 ms are outside the engine's hot path")
     model = get_speaker_model(configs["model"])(precision=configs.get("precision"), **configs["model_args"])
+    resample_rate, _ = frontend_args(test_conf, model.feat_dim)
     load_checkpoint(model, model_path)
     device = torch.device("cuda")
     model.to(device).eval()
@@ -215,7 +230,7 @@ def extract(config="conf/config.yaml", **kwargs):
                 keys_q.append(keys)
                 yield torch.from_numpy(arr).pin_memory()
 
-        for embs in model.extract_stream(host_batches()):
+        for embs in model.extract_stream(host_batches(), sample_rate=resample_rate):
             keys = keys_q.pop(0)
             for k, e in zip(keys, embs.numpy()):
                 writer(k, e)

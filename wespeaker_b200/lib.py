@@ -92,6 +92,11 @@ _PROTOS = {
     "ws_engine_last_launches": (C.c_longlong, [c_engine_p]),
     "ws_engine_destroy": (None, [c_engine_p]),
     "ws_fbank_num_frames": (C.c_int, [C.c_int]),
+    "ws_fbank_num_frames_at": (C.c_int, [C.c_int, C.c_int]),
+    "ws_fbank_at": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int,
+                              C.c_void_p, C.c_void_p]),
+    "ws_fbank_ragged_at": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_char_p,
+                                     C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ws_fbank": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_void_p,
                            C.c_void_p]),
     "ws_fbank_ragged": (C.c_int, [C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_char_p,

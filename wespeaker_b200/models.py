@@ -19,6 +19,7 @@ from collections import OrderedDict, namedtuple
 import numpy as np
 import torch
 
+from . import frontend as _frontend
 from . import lib as _lib
 from .synthetic import (CAMPP_NAMES, DEFAULT_MODEL_ARGS, ECAPA_NAMES, GEMINI_NAMES, RES2NET_NAMES, RESNET_NAMES, SIMAM_NAMES,
                         XVEC_NAMES, state_dict_spec)
@@ -217,6 +218,13 @@ class B200SpeakerModel(torch.nn.Module):
             return self._device.index
         return torch.cuda.current_device() if torch.cuda.is_available() else 0
 
+    def _wav_engine(self, dev_index: int, sample_rate: int):
+        """The engine on `dev_index`, its waveform entry points set to `sample_rate` (their fbank writes feat_dim bins)."""
+        sr, _ = _frontend.check_rate_bins(sample_rate, self.feat_dim)
+        h = self._ensure_engine(dev_index)
+        _lib.check(_lib.load().ws_engine_set_option(h, b"sample_rate", sr), "ws_engine_set_option")
+        return h
+
     # ------------------------------------------------------------------ forward paths
     def embed(self, features: torch.Tensor) -> torch.Tensor:
         """(B,T,feat_dim) float32 -> (B,embed_dim) float32 on the same device class as the input."""
@@ -249,9 +257,10 @@ class B200SpeakerModel(torch.nn.Module):
         # Callers use [-1].
         return torch.tensor(0.0), emb
 
-    def extract_from_wav(self, wav: torch.Tensor, window_type: str = "hamming", return_feats: bool = False):
-        """wav: (B,N) float32 (int16 range, i.e. ``wav * (1 << 15)``) or int16 PCM, CUDA or host.
-        fbank (dither 0) + CMN + forward entirely on the GPU."""
+    def extract_from_wav(self, wav: torch.Tensor, window_type: str = "hamming", return_feats: bool = False,
+                         sample_rate: int = 16000):
+        """wav: (B,N) float32 (int16 range, i.e. ``wav * (1 << 15)``) or int16 PCM at sample_rate (8000 or 16000), CUDA or
+        host.  fbank (feat_dim bins, dither 0) + CMN + forward entirely on the GPU."""
         if wav.dim() != 2:
             raise ValueError("wav must be (B, N)")
         L = _lib.load()
@@ -262,28 +271,28 @@ class B200SpeakerModel(torch.nn.Module):
         B, N = wav.shape
         if wav.is_cuda:
             idx = wav.device.index
-            h = self._ensure_engine(idx)
+            h = self._wav_engine(idx, sample_rate)
             out = torch.empty((B, self.embed_dim), dtype=torch.float32, device=wav.device)
-            T = L.ws_fbank_num_frames(N)
-            feats = torch.empty((B, T, 80), dtype=torch.float32, device=wav.device) if return_feats else None
+            T = _frontend.num_frames(N, sample_rate)
+            feats = torch.empty((B, T, self.feat_dim), dtype=torch.float32, device=wav.device) if return_feats else None
             with torch.cuda.device(idx):
                 _lib.check(L.ws_engine_extract_wav(h, wav.data_ptr(), is_i16, N, N, B, window_type.encode(),
                                                    out.data_ptr(), feats.data_ptr() if return_feats else None,
                                                    _lib.cur_stream_ptr(idx)), "ws_engine_extract_wav")
             return (out, feats) if return_feats else out
-        h = self._ensure_engine(self._dev_index())
+        h = self._wav_engine(self._dev_index(), sample_rate)
         out = torch.empty((B, self.embed_dim), dtype=torch.float32)
         _lib.check(L.ws_engine_extract_wav_host(h, wav.data_ptr(), is_i16, N, B, window_type.encode(),
                                                 out.data_ptr()), "ws_engine_extract_wav_host")
         return out
 
-    def extract_stream(self, host_batches, window_type: str = "hamming", depth: int = 4):
+    def extract_stream(self, host_batches, window_type: str = "hamming", depth: int = 4, sample_rate: int = 16000):
         """Pipelined extraction over an iterable of HOST waveform batches ((B,N) int16 or int16-range float32, ideally
         pinned).  Yields one pinned CPU (B, embed_dim) tensor per batch, in order.  The H2D copy of batch i+1 overlaps
         the kernels of batch i (`depth` <= 4 staging slots inside the C ABI) — the analogue of the reference's DataLoader
         prefetching (extract.py:99-103)."""
         L = _lib.load()
-        h = self._ensure_engine(self._dev_index())
+        h = self._wav_engine(self._dev_index(), sample_rate)
         pending = []  # (slot, wav_keepalive, pinned_out)
         slot = 0
         pool = getattr(self, "_pinned_out", None)
@@ -368,7 +377,8 @@ class B200SpeakerModel(torch.nn.Module):
                        "ws_engine_forward_masked")
         return out
 
-    def extract_from_wav_padded(self, wavs: torch.Tensor, n_samples, window_type: str = "hamming") -> torch.Tensor:
+    def extract_from_wav_padded(self, wavs: torch.Tensor, n_samples, window_type: str = "hamming",
+                                sample_rate: int = 16000) -> torch.Tensor:
         """(B, Nmax) waveforms (int16 or int16-range float32) with `n_samples[b]` valid samples each -> (B, embed_dim):
         fbank, CMN over each utterance's own frames, masked forward."""
         L = _lib.load()
@@ -379,7 +389,7 @@ class B200SpeakerModel(torch.nn.Module):
         w = w.contiguous() if is_i16 else w.float().contiguous()
         B, N = w.shape
         idx = w.device.index
-        h = self._ensure_engine(idx)
+        h = self._wav_engine(idx, sample_rate)
         n = torch.as_tensor(n_samples, dtype=torch.int32).to(w.device).contiguous()
         nmax = int(n.max().item())
         out = torch.empty((B, self.embed_dim), dtype=torch.float32, device=w.device)
@@ -435,11 +445,14 @@ class B200SpeakerModel(torch.nn.Module):
             return x
         return self._run_buckets(feats_list, lambda f: int(f.shape[0]), torch.stack, launch, max_batch, device)
 
-    def extract_from_wav_list(self, wavs, window_type: str = "hamming", max_batch: int = 64, device=None):
+    def extract_from_wav_list(self, wavs, window_type: str = "hamming", max_batch: int = 64, device=None,
+                              sample_rate: int = 16000):
         """Same bucketing for raw waveforms (1-D tensors of different lengths, int16 or int16-range float32)."""
         if len(wavs) == 0:
             return torch.empty((0, self.embed_dim))
         wt = window_type.encode()
+        dev = torch.device(device) if device is not None else wavs[0].device
+        self._wav_engine(dev.index if dev.type == "cuda" and dev.index is not None else self._dev_index(), sample_rate)
 
         def launch(L, h, x, o, st):
             is_i16 = 1 if x.dtype == torch.int16 else 0
@@ -460,7 +473,7 @@ class B200SpeakerModel(torch.nn.Module):
         return g
 
     def extract_from_wav_list_ragged(self, wavs, window_type: str = "hamming", max_batch: int = 64, grid_ratio: float = 1.15,
-                                     device=None) -> torch.Tensor:
+                                     device=None, sample_rate: int = 16000) -> torch.Tensor:
         """Waveforms of ARBITRARY lengths (1-D tensors, int16 or int16-range float32) -> (N, embed_dim) in input order.
         The PCM is concatenated once (no padded copies); utterances are grouped by the frame grid above into length-masked
         buckets of <= max_batch (B rounded up to 8 by repeating an utterance, so the set of (B, T) plans stays small), each
@@ -475,14 +488,15 @@ class B200SpeakerModel(torch.nn.Module):
             dev = torch.device("cuda", self._dev_index())
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         ns = [int(w.numel()) for w in wavs]
-        if min(ns) < 400:
-            raise ValueError("every waveform must hold at least one 25 ms frame (400 samples at 16 kHz)")
+        flen, shift = _frontend.frame_geometry(sample_rate)
+        if min(ns) < flen:
+            raise ValueError(f"every waveform must hold at least one 25 ms frame ({flen} samples at {sample_rate} Hz)")
         is_i16 = 1 if all(w.dtype == torch.int16 for w in wavs) else 0
         flat = torch.cat([(w if is_i16 else w.float()).reshape(-1).to(dev) for w in wavs])
         starts = np.concatenate([[0], np.cumsum(ns)[:-1]]).astype(np.int64)
         cells = {}
         for i, n in enumerate(ns):
-            cells.setdefault(self.frame_grid(1 + (n - 400) // 160, grid_ratio), []).append(i)
+            cells.setdefault(self.frame_grid(1 + (n - flen) // shift, grid_ratio), []).append(i)
         slots, batches = [], []                      # slots: utterance index per launched row; batches: (rows, Tgrid)
         for tg in sorted(cells, reverse=True):
             members = cells[tg]
@@ -498,14 +512,14 @@ class B200SpeakerModel(torch.nn.Module):
         out = torch.empty((len(slots), self.embed_dim), dtype=torch.float32, device=dev)
         first = np.full(len(wavs), -1, dtype=np.int64)
         first[slots_np[::-1]] = np.arange(len(slots) - 1, -1, -1)            # first launched row of each utterance
-        h = self._ensure_engine(idx)
+        h = self._wav_engine(idx, sample_rate)
         wt = window_type.encode()
         with torch.cuda.device(idx):
             st = _lib.cur_stream_ptr(idx)
             pos = 0
             for rows, tg in batches:
                 _lib.check(L.ws_engine_extract_wav_ragged_async(h, flat.data_ptr(), is_i16, offs.data_ptr() + 8 * pos,
-                                                                nsd.data_ptr() + 4 * pos, (tg - 1) * 160 + 400, rows, wt,
+                                                                nsd.data_ptr() + 4 * pos, (tg - 1) * shift + flen, rows, wt,
                                                                 out.data_ptr() + 4 * self.embed_dim * pos, st),
                            "ws_engine_extract_wav_ragged_async")
                 pos += rows

@@ -66,7 +66,8 @@ class Speaker:
         self.window_type = window_type
 
     def set_resample_rate(self, resample_rate: int):
-        self.resample_rate = resample_rate
+        """The rate audio is resampled to before fbank: 16000 or 8000 (the engine's fbank runs at those two)."""
+        self.resample_rate = frontend.check_rate_bins(resample_rate)[0]
 
     def set_vad(self, apply_vad: bool):
         if apply_vad:
@@ -88,11 +89,9 @@ class Speaker:
         self.diar_subseg_cmn = subseg_cmn
 
     def compute_features(self, wavform: torch.Tensor, sample_rate: int = 16000, cmn: bool = True):
-        """`cli/speaker.py:90-106`: (C,N) waveform -> (1,T,80) features on the GPU."""
-        if sample_rate != 16000:
-            raise NotImplementedError("16 kHz only")
+        """`cli/speaker.py:90-106`: (C,N) waveform at sample_rate (8000 or 16000) -> (1,T,80) features on the GPU."""
         w = wavform[:1].to(self._cuda_device())
-        return fbank_batch(w, window_type=self.window_type, cmn=cmn)
+        return fbank_batch(w, window_type=self.window_type, cmn=cmn, sample_rate=sample_rate, num_mel_bins=80)
 
     def _cuda_device(self):
         return self.device if self.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
@@ -117,10 +116,8 @@ class Speaker:
         """`cli/speaker.py:130-167`: fused fbank + CMN + forward; returns a CPU (E,) tensor."""
         pcm = pcm.to(torch.float)[:1].to(self._cuda_device())
         if sample_rate != self.resample_rate:   # cli/speaker.py:157-159: torchaudio.transforms.Resample, here on the device
-            if self.resample_rate != 16000:
-                raise NotImplementedError("the fbank kernel is built for 16 kHz features (resample_rate)")
             pcm = frontend.resample(pcm, sample_rate, self.resample_rate)
-        emb = self.model.extract_from_wav(pcm, window_type=self.window_type)
+        emb = self.model.extract_from_wav(pcm, window_type=self.window_type, sample_rate=self.resample_rate)
         return emb[0].to(torch.device("cpu"))
 
     def extract_embedding_list(self, scp_path: str):
@@ -133,8 +130,9 @@ class Speaker:
         return names, embeddings
 
     def extract_embedding_batch(self, pcm_batch: torch.Tensor):
-        """Addition: (B,N) equal-length int16/float waveforms -> (B,E) CUDA tensor in one fused pass."""
-        return self.model.extract_from_wav(pcm_batch.to(self._cuda_device()), window_type=self.window_type)
+        """Addition: (B,N) equal-length int16/float waveforms at the resample rate -> (B,E) CUDA tensor in one fused pass."""
+        return self.model.extract_from_wav(pcm_batch.to(self._cuda_device()), window_type=self.window_type,
+                                           sample_rate=self.resample_rate)
 
     def compute_similarity(self, audio_path1: str, audio_path2: str) -> float:
         """`cli/speaker.py:180-186`."""

@@ -37,25 +37,25 @@ def chunk_frame_index(num_frames: int, num_chunk_frames: int) -> np.ndarray:
 
 class SpeakerEngine:
     """`SpeakerEngine(model_path, feat_dim, sample_rate, embedding_size, SamplesPerChunk)` with the model object in place
-    of the ONNX path.  `fbank_fn(wav (1,N) int16/float tensor) -> (T,80)` and `embed_fn(feats (B,T,80)) -> (B,E)` default
-    to the GPU frontend and the engine forward; tests inject the CPU oracle to check the host logic."""
+    of the ONNX path.  `fbank_fn(wav (1,N) int16/float tensor) -> (T,feat_dim)` and `embed_fn(feats (B,T,feat_dim)) -> (B,E)`
+    default to the GPU frontend (feat_dim bins at sample_rate, 8000 or 16000) and the engine forward; tests inject the CPU
+    oracle to check the host logic."""
 
     def __init__(self, model, feat_dim: int = 80, sample_rate: int = 16000, embedding_size: int | None = None,
                  samples_per_chunk: int = 32000, fbank_fn=None, embed_fn=None):
-        if feat_dim != 80 or sample_rate != 16000:
-            raise NotImplementedError("80-bin fbank at 16 kHz only (the reference runtime's configuration)")
+        from .frontend import check_rate_bins
+        self.sample_rate, self.feat_dim = check_rate_bins(sample_rate, feat_dim)
         self.model = model
-        self.sample_rate = sample_rate
         self.per_chunk_samples = samples_per_chunk
         self._embedding_size = embedding_size
         self._fbank = fbank_fn or self._gpu_fbank
         self._embed = embed_fn or self._gpu_embed
 
     # ---- defaults: the GPU path
-    @staticmethod
-    def _gpu_fbank(wav):
+    def _gpu_fbank(self, wav):
         from .frontend import fbank_batch
-        return fbank_batch(wav.cuda(), window_type="hamming", cmn=False)[0]   # C++ frontend: hamming (fbank.h:90-95)
+        return fbank_batch(wav.cuda(), window_type="hamming", cmn=False, sample_rate=self.sample_rate,   # C++ frontend: hamming
+                           num_mel_bins=self.feat_dim)[0]                                                # (fbank.h:90-95)
 
     def _gpu_embed(self, feats):
         out = self.model(feats)
@@ -69,7 +69,7 @@ class SpeakerEngine:
         return 1 + (self.per_chunk_samples - ms * 25) // (ms * 10)          # speaker_engine.cc:97-99
 
     def extract_feature(self, pcm) -> torch.Tensor:
-        """`ExtractFeature`: (N,) or (1,N) int16 / int16-range float samples -> (nchunk, T, 80) un-normalised chunks."""
+        """`ExtractFeature`: (N,) or (1,N) int16 / int16-range float samples -> (nchunk, T, feat_dim) un-normalised chunks."""
         wav = torch.as_tensor(pcm)
         wav = wav[None] if wav.dim() == 1 else wav[:1]
         feats = self._fbank(wav)
