@@ -149,10 +149,14 @@ class TwoCovPLDA:
 
     def score_matrix(self, enroll_t, test_t, counts=1, out: torch.Tensor | None = None,
                      out_dtype=torch.float32) -> torch.Tensor:
-        """All-pairs LLR (N,M).  ``counts`` = int (constant n, K=D GEMM) or (N,) int array (K=2D GEMM)."""
+        """All-pairs LLR (N,M).  ``counts`` = int (constant n, K=D GEMM) or (N,) int array (K=2D GEMM).
+        ``out``: a float32 or float64 (N,M) CUDA tensor on this PLDA's device whose rows are unit-stride and do not
+        overlap (stride(1) == 1, stride(0) >= M); the kernel writes it through its data pointer and row stride."""
+        N, M = int(enroll_t.shape[0]), int(test_t.shape[0])
+        if out is not None:
+            self._check_out(out, N, M)
         e = self._cuda(enroll_t, torch.float64)
         t = self._cuda(test_t, torch.float64)
-        N, M = e.shape[0], t.shape[0]
         if out is None:
             out = torch.empty((N, M), dtype=out_dtype, device=e.device)
         if N == 0 or M == 0:
@@ -168,6 +172,20 @@ class TwoCovPLDA:
                 M, out.data_ptr(), 1 if out.dtype == torch.float64 else 0, out.stride(0),
                 _lib.cur_stream_ptr(self._dev())), "ws_plda_score_matrix")
         return out
+
+    def _check_out(self, out, N, M):
+        """Refuse an ``out`` the kernel would write wrongly: another dtype would be written as fp32, fewer rows or
+        overlapping rows past or over other data, a non-unit column stride in the wrong layout, a host or other-device
+        tensor through a pointer the kernel cannot use."""
+        if out.dtype not in (torch.float32, torch.float64):
+            raise ValueError(f"score_matrix: out must be float32 or float64, got {out.dtype}")
+        if tuple(out.shape) != (N, M):
+            raise ValueError(f"score_matrix: out has shape {tuple(out.shape)}, the scores are ({N}, {M})")
+        if out.stride(1) != 1 or out.stride(0) < M:
+            raise ValueError(f"score_matrix: out needs stride(1) == 1 and stride(0) >= {M}, got strides {out.stride()}")
+        dev = self._dev()
+        if not out.is_cuda or out.device.index != dev:
+            raise ValueError(f"score_matrix: out is on {out.device}, this PLDA scores on cuda:{dev}")
 
     def score_trials(self, enroll_t, test_t, enroll_idx, test_idx, counts=1) -> torch.Tensor:
         e = self._cuda(enroll_t, torch.float64)
