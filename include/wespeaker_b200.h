@@ -39,7 +39,7 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
  * against the plan builder (missing keys, shapes, kernel envelopes) on a host without a GPU.  Every compute entry point
  * returns an error on such an engine. */
 int ws_engine_create_plan_check(const char* model_name, const char* precision, int feat_dim, int embed_dim, ws_engine** out);
-/* options: "two_emb_layer", "emb_bn" (model_args), "cuda_graph" (default 1), "force_simt" (debug cross-check),
+/* options: "two_emb_layer", "emb_bn" (model_args), "cuda_graph" (default 1),
  * "sample_rate" (8000 or 16000, default 16000: the rate of the waveforms the extract_wav entry points receive; their fbank
  * writes feat_dim mel bins, 4 <= feat_dim <= 128; any other rate is refused - resample first, as the reference does),
  * "tc_version" (2: persistent / TMA-store tensor-core kernel, 3 (default): + weight-sharing CTA clusters on the large layers;

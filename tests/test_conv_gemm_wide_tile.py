@@ -7,7 +7,6 @@ The operator shapes are large enough that the wide tile is taken under the shape
 resident-cluster count: with x = (256-wide tiles) / (resident clusters) >= 5 the rule 20 r256 <= 11 r128 always holds."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -118,12 +117,14 @@ def test_wide_tile_matches_narrow_tile(path, prec, epi):
 
 @pytest.mark.gpu
 def test_wide_tile_matches_narrow_tile_cluster4():
-    """Clusters of four (WS_TC3_CL=4 is read once per process, so this runs in a subprocess)."""
-    env = dict(os.environ, WS_TC3_CL="4")
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__)]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
-    assert "cluster4 ok" in r.stdout
+    """Clusters of four (WS_TC3_CL=4, read whenever a conv op is built) for every precision and epilogue."""
+    os.environ["WS_TC3_CL"] = "4"
+    try:
+        for prec in DT:
+            for epi in EPIS:
+                _check_wide_vs_narrow(prec, 3, epi)
+    finally:
+        os.environ.pop("WS_TC3_CL", None)
 
 
 @pytest.mark.gpu
@@ -166,11 +167,3 @@ def test_ecapa1024_plan_uses_wide_tile_on_the_dense_1x1_convs():
     shapes = sorted(a.split(" pos=")[1] for a, _ in changed)
     assert shapes == ["51200 K=1024 N=1024"] * 6 + ["51200 K=3072 N=1536", "51200 K=400 N=1024"], shapes
     assert [f for _, f in wide] == [f for _, f in narrow]
-
-
-if __name__ == "__main__":
-    # the cluster-of-four cases (run by test_wide_tile_matches_narrow_tile_cluster4 with WS_TC3_CL=4)
-    for prec in DT:
-        for epi in EPIS:
-            _check_wide_vs_narrow(prec, 3, epi)
-    print("cluster4 ok")

@@ -1,4 +1,4 @@
-"""CUDA-event timing of conv shapes x tuning knobs through ws_conv (no profiler)."""
+"""CUDA-event timing of conv shapes through ws_conv (no profiler), with the default N tile and with WS_TC2_MAX_BN=128."""
 import ctypes as C, os, sys, itertools
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -42,8 +42,7 @@ if __name__ == "__main__":
         B, T, ci, co, k, d = shapes[name]
         for tcv in (2, 3):
             for knobs in ({}, {"WS_TC2_MAX_BN": "128"}):
-                if k == 1 and "WS_TILE_BT" in knobs: continue
-                for kk in ("WS_TILE_BT", "WS_TC2_MAX_STAGES", "WS_TC2_MAX_BN"): os.environ.pop(kk, None)
+                os.environ.pop("WS_TC2_MAX_BN", None)
                 os.environ.update(knobs)
                 ms, tf = time_conv(B, T, ci, co, k, d, tcv, res=(name == "res2"))
                 print(f"{name:8s} tc{tcv} {str(knobs):34s} {ms*1e3:8.1f} us {tf:7.1f} TF/s", flush=True)

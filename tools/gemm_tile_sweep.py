@@ -6,8 +6,8 @@ ECAPA-TDNN-1024 bf16 at B=256, T=200 (51 200 positions):
     1024 -> 1024, bias + ReLU              (se_res2block.0)
     1024 -> 1024, bias + ReLU + BN + SE column sums  (se_res2block.2)
     3072 -> 1536, bias + ReLU              (conv)
-under every tile setting the code can select: cluster size CL = 1 (use_tc=2), 2 and 4 (use_tc=3, WS_TC3_CL; read once per
-process, so each setting runs in a subprocess) and N-tile caps WS_TC2_MAX_BN = 64, 128, 256.
+under every tile setting the code can select: cluster size CL = 1 (use_tc=2), 2 and 4 (use_tc=3, WS_TC3_CL) and N-tile
+caps WS_TC2_MAX_BN = 64, 128, 256, each setting in a subprocess of its own.
 
 Per run it prints ms per launch, TFLOP/s, and the operand bytes each launch pulls from L2 computed from shapes:
 tiles x (128 + bn / CL) x K x 2 B (each CTA loads its 128-position A tile and 1/CL of the bn-row weight tile, which TMA

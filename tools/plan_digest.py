@@ -50,9 +50,8 @@ def cases():
         for opt in ("res2_fused", "astp_fused", "se_fused", "se_colsum"):
             out.append(("ECAPA_TDNN_c1024", prec, 2, 200, False, {}, {opt: 0}))
     for name in ("ResNet34", "ResNet50", "ERes2Net34_Base", "SimAM_ResNet34_ASP", "Gemini_DF_ResNet60", "CAMPPlus"):
-        for opt in ("conv3x3", "conv3x3_strided"):
-            for masked in (False, True):
-                out.append((name, "fp16", 2, 200, masked, {}, {opt: 0}))
+        for masked in (False, True):
+            out.append((name, "fp16", 2, 200, masked, {}, {"conv3x3": 0}))
     for opt in ("cam_fused", "cam_block"):
         out.append(("CAMPPlus", "bf16", 2, 200, False, {}, {opt: 0}))
     for T in (998, 2400):
@@ -62,9 +61,8 @@ def cases():
             out.append((name, prec, 2, 200, False, {"two_emb_layer": True}, {}))
     for prec in ("tf32x3", "bf16"):
         out.append(("ECAPA_TDNN_c512", prec, 2, 200, False, {"emb_bn": True}, {}))
-    for opts in ({"force_simt": 1}, {"tc_version": 2}):
-        for prec in ("tf32x3", "bf16"):
-            out.append(("ResNet34", prec, 2, 200, False, {}, opts))
+    for prec in ("tf32x3", "bf16"):
+        out.append(("ResNet34", prec, 2, 200, False, {}, {"tc_version": 2}))
     return out
 
 

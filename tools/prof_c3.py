@@ -1,17 +1,15 @@
-"""Time the halo-resident 3x3 conv (ws_conv, use_tc=4) at several shapes in ONE process; WS_C3_PROF=1 prints the kernel's
-phase profile, WS_C3_DBG knocks out roles.  usage: prof_c3.py "B F T C" ... [--dbg 0,11] [--tc 4,3] [--prof]"""
+"""Time the halo-resident 3x3 conv (ws_conv, use_tc=4) at several shapes in ONE process.
+usage: prof_c3.py "B F T C" ... [--tc 4,3]"""
 import os, sys, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from wespeaker_b200 import lib
 args = sys.argv[1:]
-dbgs, tcs, prof = [0], [4], False
+tcs = [4]
 shapes = []
 i = 0
 while i < len(args):
-    if args[i] == "--dbg": dbgs = [int(x) for x in args[i + 1].split(",")]; i += 2
-    elif args[i] == "--tc": tcs = [int(x) for x in args[i + 1].split(",")]; i += 2
-    elif args[i] == "--prof": prof = True; i += 1
+    if args[i] == "--tc": tcs = [int(x) for x in args[i + 1].split(",")]; i += 2
     else: shapes.append(tuple(int(x) for x in args[i].split())); i += 1
 if not shapes:
     shapes = [(64, 80, 200, 32), (64, 40, 100, 64), (64, 20, 50, 128)]
@@ -52,14 +50,8 @@ def run(B, F, T, Cc, use_tc, with_res, n=10):
 for (B, F, T, Cc) in shapes:
     fl = 2.0 * B * F * T * 9 * Cc * Cc
     for tc in tcs:
-        for dbg in (dbgs if tc == 4 else [0]):
-            for with_res in (0, 1):
-                os.environ["WS_C3_DBG"] = str(dbg)
-                if prof and tc == 4:
-                    os.environ["WS_C3_PROF"] = "1"
-                    run(B, F, T, Cc, tc, with_res, n=1)
-                    os.environ.pop("WS_C3_PROF")
-                ms = run(B, F, T, Cc, tc, with_res)
-                by = B * F * T * Cc * 2 * (3 if with_res else 2)
-                print(f"conv3x3 B{B} F{F} T{T} C{Cc} use_tc={tc} dbg={dbg} res={with_res}: {ms*1e3:.1f} us, {fl/ms/1e9:.0f} TFLOP/s, "
-                      f"{by/ms/1e6:.0f} GB/s algorithmic", flush=True)
+        for with_res in (0, 1):
+            ms = run(B, F, T, Cc, tc, with_res)
+            by = B * F * T * Cc * 2 * (3 if with_res else 2)
+            print(f"conv3x3 B{B} F{F} T{T} C{Cc} use_tc={tc} res={with_res}: {ms*1e3:.1f} us, {fl/ms/1e9:.0f} TFLOP/s, "
+                  f"{by/ms/1e6:.0f} GB/s algorithmic", flush=True)

@@ -40,9 +40,6 @@ __device__ __forceinline__ float cvt16(uint32_t v) {
     return __half2float(__ushort_as_half((unsigned short)v));
 }
 
-#define AP_T(x) const long long x = p.prof ? clock64() : 0
-#define AP_ADD(i, v) do { if (p.prof && lane == 0) p.prof[(size_t)blockIdx.x * 16 + (i)] += (v); } while (0)
-
 template <int DT>
 __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __grid_constant__ WsAstpParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -64,7 +61,6 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
     }
     __syncthreads();
     const int nblk = p.C / 128, upb = nblk / p.g, nunits = p.B * upb;
-    AP_T(k0);
 
     if (warp == 0) {
         // ================================ TMA producer ================================
@@ -75,9 +71,7 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
                 const int Tb = p.lens ? max(1, min(p.T, p.lens[b])) : p.T;
                 const int nch = (Tb + 255) >> 8;
                 auto load_h = [&](int ch) {
-                    AP_T(a0);
                     mbar_wait(bar_hempty, (h_it & 1u) ^ 1u);
-                    AP_T(a1); AP_ADD(0, a1 - a0);
                     mbar_expect_tx(bar_hfull, 2u * kHPanelBytes);
                     tma_load_3d(hbuf, &p.hmap, bar_hfull, 0, ch * 256, b);
                     tma_load_3d(hbuf + kHPanelBytes, &p.hmap, bar_hfull, 64, ch * 256, b);
@@ -89,9 +83,7 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
                         if (nch > 1) load_h(ch);
                         if (ch == 0) {
                             const uint32_t ws = w_it & 1u;
-                            AP_T(a2);
                             mbar_wait(bar_wempty + 8 * ws, ((w_it >> 1) & 1u) ^ 1u);
-                            AP_T(a3); AP_ADD(1, a3 - a2);
                             mbar_expect_tx(bar_wfull + 8 * ws, 2u * kWPanelBytes);
                             const uint32_t dst = wbuf + ws * 2u * kWPanelBytes;
                             tma_load_2d(dst, &p.wmap, bar_wfull + 8 * ws, 0, (blk0 + j) * 128);
@@ -121,9 +113,7 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
             const int b = u / upb, blk0 = (u % upb) * p.g;
             const int Tb = p.lens ? max(1, min(p.T, p.lens[b])) : p.T;
             const int nch = (Tb + 255) >> 8;
-            AP_T(m0);
             if (nch == 1) { mbar_wait(bar_hfull, h_it & 1u); ++h_it; }
-            AP_T(m1); AP_ADD(2, m1 - m0);
             for (int j = 0; j < p.g; ++j) {
                 const uint32_t ws = w_it & 1u;
                 float m[2] = {-INFINITY, -INFINITY}, s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
@@ -223,8 +213,6 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
             if (nch == 1 && (threadIdx.x & 127) == 0) mbar_arrive(bar_hempty);
         }
     }
-    __syncthreads();
-    if (warp == 2) { AP_T(k1); AP_ADD(10, k1 - k0); }
 }
 
 }  // namespace

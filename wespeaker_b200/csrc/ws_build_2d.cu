@@ -18,7 +18,7 @@ View basic_block(Builder& b, const std::string& p, const View& x, int cout, int 
     const View h = hbuf.shaped(x.B, Fo, To, cout), o = obuf.shaped(x.B, Fo, To, cout);
     if (!b.conv3x3(x, h, b.w.act("w:" + p + ".conv1", w1), b.w.f32("bnh:" + p + ".bn1", h1), WS_ACT_RELU, sf, st_, lvl)) return none;
     const bool has_sc = b.e.sd.count(p + ".shortcut.0.weight") != 0;
-    if (b.halo3x3(1, 1) && (cout == 32 || cout == 64 || cout == 128)) {
+    if (b.halo3x3() && (cout == 32 || cout == 64 || cout == 128)) {
         // conv2 on the halo-resident kernel: the 1x1 strided shortcut conv (+ its BN) is written to `o` first and then
         // read back as the residual, in place (each output element is read and written by the same CTA step).  conv2's op is
         // built first: if the shape is outside the kernel's envelope nothing has been emitted yet.  (The channel counts the

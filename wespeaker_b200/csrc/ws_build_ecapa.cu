@@ -36,7 +36,7 @@ bool build_ecapa(Builder& b) {
     View xin = out1;
     float* se_colsum = nullptr;
     if (e.use_tc >= 2 && e.act_dt != WS_F32 && !e.split && T >= 128 && (C == 512 || C == 1024) && e.opt("se_fused", 1) &&
-        e.opt("se_colsum", 1) && getenv("WS_EPI_GENERIC") == nullptr && !b.p.masked)   // (column sums would include padding rows)
+        e.opt("se_colsum", 1) && !b.p.masked)   // (column sums would include padding rows)
         se_colsum = b.f32((size_t)2 * (((size_t)B * T + 63) / 64) * C);
     for (int L = 2; L <= 4 && b.good(); ++L) {
         const int d = L;

@@ -74,8 +74,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    const long long tk0 = clock64();
-#define CAM_TS(i) do { if (p.prof && blockIdx.x == 0 && et == 0 && l == p.l0) p.prof[i] = clock64() - tk0; } while (0)
 
     if (warp == 0) {
         // ================================ TMA producer ================================
@@ -123,7 +121,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
             }
             if (et < 128) s_bias2[et] = __ldg(L->bias2 + et);
             epi_bar_sync();
-            CAM_TS(0);
             for (int tile = 0; tile < nmt; ++tile) {
                 float acc[64];
                 for (int kp = 0; kp < npan; ++kp) {
@@ -183,7 +180,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
             if ((threadIdx.x & 127) == 0) mbar_arrive(bar_acc1);   // the ring front may take the local-conv weights
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             epi_bar_sync();
-            CAM_TS(3);
             // ---- context: per-segment column sums of the STORED (rounded) h, like the unfused gate kernel reads them.
             //      thread = (16-byte chunk of 8 channels, 1 of 16 row groups); the two row groups of a warp are combined by a
             //      shuffle, the 8 warps through shared memory: deterministic summation order.
@@ -222,7 +218,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
                 }
                 (void)tot8;
             }
-            CAM_TS(4);
             if (et < 128) {
                 float tot = 0.f;
                 for (int sg = 0; sg < nseg; ++sg) tot += s_ctx[sg * 128 + et];
@@ -233,7 +228,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
                 }
             }
             epi_bar_sync();
-            CAM_TS(5);
             {   // hidden = ReLU(W1 ctx + b1): thread = (output j, quarter of the 128 inputs); W1 transposed -> coalesced; all
                 // 32 weight loads of a thread are in flight at once (they are L2 hits, ~700 cycles each if serialised)
                 const int j = et & 63, qt = et >> 6;
@@ -255,7 +249,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
             for (int i = 0; i < 8; ++i) w2v[i] = __ldg(L->w2c_t + (gp * 8 + i) * 32 + gg);
             const float b2v = __ldg(L->b2c + gg);
             epi_bar_sync();
-            CAM_TS(6);
             for (int o = et; o < nseg * 64; o += 256) {
                 const int sg = o >> 6, j = o & 63;
                 float a = __ldg(L->b1c + j);
@@ -264,7 +257,6 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
                 s_hid[sg * 64 + j] = fmaxf(a, 0.f);
             }
             epi_bar_sync();
-            CAM_TS(7);
             for (int sg = 0; sg < nseg; ++sg) {     // gate partials: thread = (output g, eighth of the 64 hidden units)
                 float a = 0.f;
 #pragma unroll
@@ -280,11 +272,9 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
                 s_gate[sg * 32 + g] = 1.f / (1.f + expf(-a));
             }
             epi_bar_sync();
-            CAM_TS(8);
             // ---- local conv: 3 dilated taps as row-shifted reads of the hidden operand buffer, K = 128 (2 panels), N = 32;
             //      epilogue 2: y = local_conv(h) * gate[segment(t)] -> 64-byte-row staging -> TMA store (clips rows >= T)
             mbar_wait(bar_wl, lph);
-            CAM_TS(9);
             for (int tile = 0; tile < nmt; ++tile) {
                 float acc2[16];
                 ws_wg::fence();
@@ -321,10 +311,8 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
             if (et == 0) {
                 for (int tile = 0; tile < nmt; ++tile) tma_store_3d(&p.omap, sOut + (uint32_t)(tile * 8192), cin, tile * 128, b);
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                CAM_TS(10);
                 asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // writes complete: the next layer may load them
                 mbar_arrive(bar_ldone);
-                CAM_TS(11);
             }
         }
     }

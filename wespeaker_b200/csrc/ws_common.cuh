@@ -306,7 +306,7 @@ struct WsTc2Params {
     int has_out2, has_epin;
     int nsplit;          // 1, or 3 = 3xTF32 error-compensated passes (x_lo*W, x*W_lo, x*W)
     int nout;            // number of output tiles staged per tile (1..4)
-    int epi_generic;     // test knob (WS_EPI_GENERIC=1): always run the generic epilogue instantiation
+    int epi_generic;     // always run the generic epilogue instantiation (ConvSpec::epi_generic, a test reference)
     int grid, smem_bytes;
     int cl;              // CTAs per cluster: 1, or 2 / 4 (ws_tc3_launch) sharing the weight tile by TMA multicast
     WsEpi epi;
@@ -324,7 +324,6 @@ struct WsAstpParams {
     int g;              // channel blocks (of 128) per work unit: H is fetched once per unit
     int grid;
     const int* lens;    // length-masked batch: frames of each utterance, or null
-    long long* prof;    // WS_ASTP_PROF: [grid][16] wait-cycle counters per role
     float var_floor;    // std = sqrt(max(var, var_floor))
 };
 
@@ -378,9 +377,7 @@ struct WsC3Params {
     int case_b;
     int total_steps;               // n_nt * n_tt * n_bg * F output-row steps, split contiguously over the CTAs
     int grid, smem_bytes;
-    long long* prof;               // tuning aid (WS_C3_PROF=1): per-CTA wait-cycle counters, 16 slots per CTA; else null
     const int* lens;               // length-masked batch: output frames of each utterance (rows behind are stored as zeros), or null
-    int dbg;                       // tuning aid (WS_C3_DBG): knock-out bits 1 = no epilogue work, 2 = no input TMA loads
 };
 
 // fused CAM++ dense layer (ws_cam_dense.cu).  One descriptor per CAMDenseTDNNLayer, device-resident (the tensor maps are
@@ -406,7 +403,6 @@ struct WsCamParams {
     int B, T, nmt, seg_len, dtype;
     int nstages, hrows;       // ring stages (32 KB each); rows per panel of the hidden operand buffer (16 + 128 * nmt)
     int grid, smem_bytes;
-    long long* prof;          // tuning aid (WS_CAM_PROF=1): phase timestamps of CTA 0, first layer; else null
     const int* lens;          // length-masked batch: frames of each utterance (statistics and padding follow them), or null
 };
 

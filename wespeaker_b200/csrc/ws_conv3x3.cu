@@ -26,10 +26,6 @@ using namespace ws_tcdev;
 constexpr int kC3Threads = 384;
 constexpr int kC3MaxSmem = 222 * 1024;
 
-// clock64 phase profile (p.prof != null): accumulate the cycles one elected thread of each role spends in each wait
-#define C3_T0() const long long t0__ = p.prof ? clock64() : 0
-#define C3_ACC(var) do { if (p.prof) var += clock64() - t0__; } while (0)
-
 // Walk over this CTA's contiguous range of output-row steps.  The (f, b group, t tile, n tile) decomposition costs integer
 // divisions only once; every role advances it incrementally (a 64-bit div/mod per step and role was ~5k cycles per step of
 // pure overhead in the first version of this kernel).
@@ -107,13 +103,10 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
         // ================================ input-row producer ================================
         if (lane == 0) {
             const uint32_t tx = (uint32_t)(p.npan * p.rows_loaded * p.row_bytes);
-            long long pw_aempty = 0;
-            const long long tstart = p.prof ? clock64() : 0;
             int slot = 0;
             uint32_t sphase = 1;                             // waits on the "previous" phase of a fresh barrier pass at once
             auto load_row = [&](int frow, int bg, int tt) {
-                { C3_T0(); mbar_wait(bar_aempty + 8 * slot, sphase); C3_ACC(pw_aempty); }
-                if (p.dbg & 2) { mbar_arrive(bar_afull + 8 * slot); if (++slot == p.R) { slot = 0; sphase ^= 1u; } return; }
+                mbar_wait(bar_aempty + 8 * slot, sphase);
                 mbar_expect_tx(bar_afull + 8 * slot, tx);
                 const int tc = tt * p.tb - 1, b0 = bg * p.nb;
                 for (int kp = 0; kp < p.npan; ++kp) {
@@ -140,7 +133,6 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
                 if (st.first || p.sf == 2) load_row(fi, st.bg, st.tt);
                 load_row(fi + 1, st.bg, st.tt);
             }
-            if (p.prof) { p.prof[blockIdx.x * 16 + 0] = pw_aempty; p.prof[blockIdx.x * 16 + 1] = clock64() - tstart; }
         }
     } else if (warp == 3) {
         // ================================ weight producer ================================
@@ -183,7 +175,7 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
         const int tap_row0 = p.st == 2 ? p.sub_rows : 0, tap_row1 = p.st == 2 ? 0 : 1, tap_row2 = p.st == 2 ? p.sub_rows + 1 : 2;
         const int R = p.R;
         const int nunits = p.n_mt * npanels_out;                 // store units per step (M tile, column panel)
-        const bool has_res = p.res != nullptr && !(p.dbg & 1);
+        const bool has_res = p.res != nullptr;
         const int nbuf = p.stg_bufs;
         // The residual panel of a unit is TMA-loaded INTO that unit's output staging panel (same box geometry and swizzle);
         // the epilogue reads it from there and overwrites it in place.  With three staging buffers the load for step s+1 is
@@ -199,8 +191,6 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
                             x.f, x.bg * p.nb);
             }
         };
-        long long mw_afull = 0, mw_wfull = 0, ew_store = 0, ew_res = 0;
-        const long long tstart = p.prof ? clock64() : 0;
         if (p.w_resident && s_beg < s_end) mbar_wait(bar_wres, 0);
         if (has_res && nbuf >= 2 && tma_thread && s_beg < s_end) issue_res(C3Iter(p, s_beg, s_end).cur(p), 0);
         int jslot = 0, wst = 0, last_nt = -1, ob = 0;    // ob == step % nbuf
@@ -208,13 +198,10 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
         for (C3Iter it(p, s_beg, s_end); !it.done(); it.next(p)) {
             const C3Step st = it.cur(p);
             const int nnew = st.first ? 3 : p.sf;        // a new image segment starts with rows f-1, f, f+1
-            {   // wait for the newly loaded rows: slot / phase of load i follow incrementally from (jslot, jphase)
-                C3_T0();
-                for (int i = 0; i < nnew; ++i) {
-                    mbar_wait(bar_afull + 8 * jslot, jphase);
-                    if (++jslot == R) { jslot = 0; jphase ^= 1u; }
-                }
-                C3_ACC(mw_afull);
+            // wait for the newly loaded rows: slot / phase of load i follow incrementally from (jslot, jphase)
+            for (int i = 0; i < nnew; ++i) {
+                mbar_wait(bar_afull + 8 * jslot, jphase);
+                if (++jslot == R) { jslot = 0; jphase ^= 1u; }
             }
             // ---- mainloop: the three input rows (runtime loop), everything inside unrolled
             int sl0 = jslot - 3 < 0 ? jslot - 3 + R : jslot - 3;        // slot of row f-1
@@ -231,7 +218,7 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
                     for (int kp = 0; kp < NPAN; ++kp, ++wblk) {
                         uint32_t b_addr;
                         if (!p.w_resident) {
-                            { C3_T0(); mbar_wait(bar_wfull + 8 * wst, wph); C3_ACC(mw_wfull); }
+                            mbar_wait(bar_wfull + 8 * wst, wph);
                             b_addr = wbuf + (uint32_t)(wst * wblk_bytes);
                         } else {
                             b_addr = wbuf + (uint32_t)(wblk * wblk_bytes);
@@ -274,7 +261,6 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
             const uint32_t sbuf = stg + (uint32_t)(ob * obuf_bytes);
             const int ob_next = ob + 1 == nbuf ? 0 : ob + 1;
             if (tma_thread) {
-                C3_T0();
                 if (nbuf == 1) {          // single staging buffer: free once the previous store has read it
                     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                     if (has_res) issue_res(st, 0);
@@ -286,62 +272,55 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
                         if (!nx.done()) issue_res(nx.cur(p), ob_next);
                     }
                 }
-                C3_ACC(ew_store);
             }
             if (st.nt != last_nt) {
                 for (int c = et; c < p.N; c += 256) spar[c] = p.bias ? __ldg(p.bias + n0 + c) : 0.f;
                 last_nt = st.nt;
             }
             epi_bar_sync();
-            if (has_res) { C3_T0(); mbar_wait(bar_rfull + 8 * ob, rph); C3_ACC(ew_res); }
-            if (!(p.dbg & 1)) {
+            if (has_res) mbar_wait(bar_rfull + 8 * ob, rph);
 #pragma unroll
-                for (int mt = 0; mt < NMT; ++mt) {
+            for (int mt = 0; mt < NMT; ++mt) {
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int r = rw + 8 * h;                       // row inside the M tile
-                        bool zero = false;
-                        if (p.lens != nullptr) {   // length-masked batch: frames behind the utterance's end are the next conv's padding
-                            const int i2 = mt * 128 + r, u = i2 / p.P, tti = i2 - u * p.P, bb = min(b0 + u, p.B - 1);
-                            zero = t0 + tti >= p.lens[bb];
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rw + 8 * h;                       // row inside the M tile
+                    bool zero = false;
+                    if (p.lens != nullptr) {   // length-masked batch: frames behind the utterance's end are the next conv's padding
+                        const int i2 = mt * 128 + r, u = i2 / p.P, tti = i2 - u * p.P, bb = min(b0 + u, p.B - 1);
+                        zero = t0 + tti >= p.lens[bb];
+                    }
+#pragma unroll
+                    for (int jg = 0; jg < NN / 8; ++jg) {
+                        const int c = 8 * jg + cq, pn = c / p.panel_cols, cc = c - pn * p.panel_cols;
+                        const uint32_t a = sbuf + (uint32_t)(mt * tile_bytes + pn * panel_stride + r * p.panel_bytes +
+                                                             (swz_chunk(cc >> 3, r, p.panel_bytes) << 4) + (cc & 7) * 2);
+                        float v0 = acc[mt][4 * jg + 2 * h] + spar[c], v1 = acc[mt][4 * jg + 2 * h + 1] + spar[c + 1];
+                        if (has_res) {
+                            uint32_t w;
+                            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(a));
+                            v0 += ws_16_to_f(w & 0xffffu, DT); v1 += ws_16_to_f(w >> 16, DT);
                         }
-#pragma unroll
-                        for (int jg = 0; jg < NN / 8; ++jg) {
-                            const int c = 8 * jg + cq, pn = c / p.panel_cols, cc = c - pn * p.panel_cols;
-                            const uint32_t a = sbuf + (uint32_t)(mt * tile_bytes + pn * panel_stride + r * p.panel_bytes +
-                                                                 (swz_chunk(cc >> 3, r, p.panel_bytes) << 4) + (cc & 7) * 2);
-                            float v0 = acc[mt][4 * jg + 2 * h] + spar[c], v1 = acc[mt][4 * jg + 2 * h + 1] + spar[c + 1];
-                            if (has_res) {
-                                uint32_t w;
-                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(a));
-                                v0 += ws_16_to_f(w & 0xffffu, DT); v1 += ws_16_to_f(w >> 16, DT);
-                            }
-                            if (p.relu) {
-                                v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
-                                if (p.relu == 2) { v0 = fminf(v0, 20.f); v1 = fminf(v1, 20.f); }   // Hardtanh(0, 20) (eres2net.py:43-52)
-                            }
-                            if (zero) { v0 = 0.f; v1 = 0.f; }
-                            // rows that are no output position (halo columns, rows past T or B) hold junk: the TMA store clips them
-                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(ws_pack2(v0, v1, DT)) : "memory");
+                        if (p.relu) {
+                            v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                            if (p.relu == 2) { v0 = fminf(v0, 20.f); v1 = fminf(v1, 20.f); }   // Hardtanh(0, 20) (eres2net.py:43-52)
                         }
+                        if (zero) { v0 = 0.f; v1 = 0.f; }
+                        // rows that are no output position (halo columns, rows past T or B) hold junk: the TMA store clips them
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(ws_pack2(v0, v1, DT)) : "memory");
                     }
                 }
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             epi_bar_sync();
             if (tma_thread) {
-                if (!(p.dbg & 1)) {
-                    for (int u = 0; u < nunits; ++u) {
-                        const int mt = u / npanels_out, pn = u - mt * npanels_out;
-                        tma_store_4d(&p.omap, sbuf + (uint32_t)(mt * tile_bytes + pn * panel_stride), n0 + pn * p.panel_cols,
-                                     p.case_b ? 0 : t0 + 128 * mt, st.f, b0);
-                    }
+                for (int u = 0; u < nunits; ++u) {
+                    const int mt = u / npanels_out, pn = u - mt * npanels_out;
+                    tma_store_4d(&p.omap, sbuf + (uint32_t)(mt * tile_bytes + pn * panel_stride), n0 + pn * p.panel_cols,
+                                 p.case_b ? 0 : t0 + 128 * mt, st.f, b0);
                 }
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                 if (nbuf == 2) {   // the other buffer (the store of step s-1) must be drained before anything lands in it
-                    C3_T0();
                     asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                    C3_ACC(ew_store);
                     if (has_res) {
                         C3Iter nx = it;
                         nx.next(p);
@@ -353,11 +332,6 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
             if (ob == 0) rph ^= 1u;
         }
         if (tma_thread) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-        if (p.prof && et == 0) {
-            p.prof[blockIdx.x * 16 + 2] = mw_afull; p.prof[blockIdx.x * 16 + 4] = mw_wfull;
-            p.prof[blockIdx.x * 16 + 6] = ew_store; p.prof[blockIdx.x * 16 + 8] = ew_res;
-            p.prof[blockIdx.x * 16 + 10] = clock64() - tstart; p.prof[blockIdx.x * 16 + 11] = s_end - s_beg;
-        }
     }
 }
 

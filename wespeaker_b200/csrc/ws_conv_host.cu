@@ -218,8 +218,6 @@ static bool tc2_geometry(const ConvSpec& s, WsTc2Params* q) {
     int B = s.B, F = s.F, T = s.T;
     const bool flat = s.dense_pointwise;
     int bt = 128, bf = 1, bb = 1;
-    const char* env_bt = getenv("WS_TILE_BT");  // tuning knob: minimum time-extent of a non-flat tile
-    const int min_bt = env_bt ? atoi(env_bt) : 1;
     if (flat) {
         T = s.B * s.F * s.T; F = 1; B = 1;
     } else {
@@ -228,7 +226,6 @@ static bool tc2_geometry(const ConvSpec& s, WsTc2Params* q) {
             for (int f = 1; t * f <= 128; f <<= 1) {
                 const int b = 128 / (t * f);
                 if (F == 1 && f != 1) continue;
-                if (t < min_bt && t < 128 && F == 1) continue;
                 const long long cost = (long long)((T + t - 1) / t) * t * ((F + f - 1) / f) * f * ((B + b - 1) / b) * b;
                 if (best < 0 || cost < best || (cost == best && t > bt)) { best = cost; bt = t; bf = f; bb = b; }
             }
@@ -280,7 +277,7 @@ static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
     q->nout = (s.split ? 2 : 1) * (q->has_out2 ? 2 : 1);
     const int nstage_bufs = q->nout + (q->has_epin ? 1 : 0);
     const int budget = ws_tc2_max_smem() - 1024;
-    { const char* eg = getenv("WS_EPI_GENERIC"); q->epi_generic = eg != nullptr && atoi(eg) != 0; }
+    q->epi_generic = s.epi_generic;
     const int mtiles = q->tiles_t * q->tiles_f * q->tiles_b;
     const int g_num_sms = ws_num_sms();
     int ncl = g_num_sms;                       // clusters (or CTAs) resident at once
@@ -306,8 +303,6 @@ static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
     const int cands[4] = {256, 128, 64, 32};
     const char* env_bn = getenv("WS_TC2_MAX_BN");
     const int max_bn = env_bn ? atoi(env_bn) : 256;
-    const char* env_st = getenv("WS_TC2_MAX_STAGES");
-    const int max_st = env_st ? atoi(env_st) : WS_TC_MAX_STAGES;
     for (int pass = 0; pass < 2 && bn == 0; ++pass)
         for (int ci = 0; ci < 4; ++ci) {
             const int c = cands[ci];
@@ -317,7 +312,7 @@ static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
             const int staging = staging_bytes(c);
             const int stage_bytes = (128 + c) * q->bk_bytes;
             const int n = (budget - staging) / stage_bytes;
-            if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > max_st ? max_st : n; break; }
+            if (n >= (pass == 0 ? 3 : 2)) { bn = c; nst = n > WS_TC_MAX_STAGES ? WS_TC_MAX_STAGES : n; break; }
         }
     if (bn == 0) {
         if (pair) return OpBuild::outside;
@@ -401,8 +396,8 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
         // big layers: clusters of CTAs on adjacent position tiles share the weight tile by TMA multicast
         auto q = std::make_shared<WsTc2Params>();
         // (two CTAs per cluster; WS_TC3_CL=4 takes four on the largest layers)
-        static const int cl_env = getenv("WS_TC3_CL") ? atoi(getenv("WS_TC3_CL")) : 2;
-        const int cl = (cl_env == 4 && (long long)spec.B * spec.F * spec.T >= 2LL * min_pos) ? 4 : 2;
+        const char* env_cl = getenv("WS_TC3_CL");
+        const int cl = (env_cl && atoi(env_cl) == 4 && (long long)spec.B * spec.F * spec.T >= 2LL * min_pos) ? 4 : 2;
         const OpBuild r = build_tc2(spec, q.get(), cl);
         if (r == OpBuild::built) {
             out->run = [q](cudaStream_t s) { return ws_tc3_launch(q.get(), s); };
@@ -431,7 +426,7 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
 OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
                      const float* shift, int w8, int dil, PlanOp* op, const int* lens) {
     // T > 256: time tiles with a 32-row halo per side cover the chain's receptive field (7 * dil rows) up to dilation 4
-    if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7 || getenv("WS_NO_RES2_FUSED"))
+    if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7)
         return OpBuild::outside;
     auto q = std::make_shared<WsRes2Params>();
     memset(q.get(), 0, sizeof(WsRes2Params));
@@ -474,7 +469,7 @@ OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float
 
 OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, const int* lens) {
     if (x.dt == WS_F32 || h.dt != x.dt || x.C % 128 != 0 || h.C != 128 || h.ld != 128 || x.F != 1 || h.F != 1 || h.T != x.T ||
-        h.B != x.B || getenv("WS_NO_ASTP_FUSED"))
+        h.B != x.B)
         return OpBuild::outside;
     auto q = std::make_shared<WsAstpParams>();
     memset(q.get(), 0, sizeof(WsAstpParams));
@@ -510,34 +505,8 @@ OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats,
     for (int g : cand) if (nblk % g == 0 && eff(g) > best) best = eff(g);
     q->g = 1;
     for (int g : cand) if (nblk % g == 0 && eff(g) >= 0.92 * best) { q->g = g; break; }
-    if (const char* eg = getenv("WS_ASTP_G")) { const int g = atoi(eg); if (g > 0 && nblk % g == 0) q->g = g; }
     const long long units = (long long)x.B * (nblk / q->g);
     q->grid = (int)(units < sms ? units : sms);
-    if (getenv("WS_ASTP_PROF")) {   // tuning aid: synchronous launch + per-role wait-cycle summary on stderr
-        long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("astp: prof buffer"); return OpBuild::error; }
-        q->prof = prof;
-        op->run = [q](cudaStream_t s) -> const char* {
-            cudaMemsetAsync(q->prof, 0, (size_t)q->grid * 16 * 8, s);
-            const char* m = ws_astp_launch(q.get(), s);
-            if (m) return m;
-            cudaStreamSynchronize(s);
-            std::vector<long long> h((size_t)q->grid * 16);
-            cudaMemcpy(h.data(), q->prof, h.size() * 8, cudaMemcpyDeviceToHost);
-            static const char* names[11] = {"prod.wait_hempty", "prod.wait_wempty", "cons.wait_hfull", "-", "-",
-                                            "-", "-", "-", "-", "-", "total"};
-            fprintf(stderr, "[astp prof] grid %d g %d:", q->grid, q->g);
-            for (int k = 0; k < 11; ++k) {
-                double acc = 0;
-                for (int c = 0; c < q->grid; ++c) acc += (double)h[(size_t)c * 16 + k];
-                fprintf(stderr, " %s=%.0f", names[k], acc / q->grid);
-            }
-            fprintf(stderr, "\n");
-            return nullptr;
-        };
-        op->label = "astp_fused (profiled)";
-        return OpBuild::built;
-    }
     op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
     if (plan_trace_mode())
         op->trace = "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) +
@@ -555,8 +524,7 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
     const int F = (Fin + 2 - 3) / stride_f + 1, T = (Tin + 2 - 3) / stride_t + 1;   // output extents
     auto chan_ok = [](int c) { return c == 32 || c == 64 || c == 128; };
     if (x.dt == WS_F32 || out.dt != x.dt || !chan_ok(Cin) || !chan_ok(Cout) || out.B != B || out.F != F || out.T != T ||
-        (stride_f != 1 && stride_f != 2) || (stride_t != 1 && stride_t != 2) || T < 1 || F < 1 || (x.ld * 2) % 16 != 0 || (out.ld * 2) % 16 != 0 || (res && (res->ld * 2) % 16 != 0) ||
-        getenv("WS_NO_CONV3X3"))
+        (stride_f != 1 && stride_f != 2) || (stride_t != 1 && stride_t != 2) || T < 1 || F < 1 || (x.ld * 2) % 16 != 0 || (out.ld * 2) % 16 != 0 || (res && (res->ld * 2) % 16 != 0))
         return OpBuild::outside;
     auto q = std::make_shared<WsC3Params>();
     memset(q.get(), 0, sizeof(WsC3Params));
@@ -604,7 +572,7 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
         const int stg_bytes = n_mt * (q->N / q->panel_cols) * q->stg_rows * q->panel_bytes;
         // three output staging buffers with a residual (its TMA load then leads its use by a full step), two without (stores
         // are never waited for), as long as a ring of >= 5 slots still fits beside them; else one
-        for (int bufs = (res != nullptr && !getenv("WS_C3_NO_3BUF")) ? 3 : 2; bufs >= 1; --bufs) {
+        for (int bufs = res != nullptr ? 3 : 2; bufs >= 1; --bufs) {
             const int fixed = bufs * stg_bytes + q->N * 4 + 2048 /* alignment slack */;
             q->w_resident = (budget - fixed - nwblk * wblk) / slot_bytes >= 5;
             q->w_stages = q->w_resident ? 0 : 3;
@@ -673,7 +641,6 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
     q->bias = bias;
     q->relu = relu;   // 0 none, 1 ReLU, 2 Hardtanh(0, 20)
     q->lens = lens;
-    if (const char* dbg = getenv("WS_C3_DBG")) q->dbg = atoi(dbg);
     char buf[200];
     snprintf(buf, sizeof buf, "conv3x3 B=%d F=%d T=%d Cin=%d Cout=%d s=%dx%d caseB=%d nb=%d n_mt=%d R=%d res=%d", q->B, q->F, q->T,
              q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
@@ -683,31 +650,6 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
         op->trace = "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) +
                     "," + (res ? tview("res", *res) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) +
                     "," + tp("lens", lens) + "}";
-    if (getenv("WS_C3_PROF")) {   // tuning aid: synchronous launch + per-role wait-cycle summary on stderr
-        long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, (size_t)q->grid * 16 * 8) != cudaSuccess) { set_err("conv3x3: prof buffer"); return OpBuild::error; }
-        cudaMemset(prof, 0, (size_t)q->grid * 16 * 8);
-        q->prof = prof;
-        op->run = [q](cudaStream_t s) -> const char* {
-            const char* m = ws_c3_launch(q.get(), s);
-            if (m) return m;
-            cudaStreamSynchronize(s);
-            std::vector<long long> h((size_t)q->grid * 16);
-            cudaMemcpy(h.data(), q->prof, h.size() * 8, cudaMemcpyDeviceToHost);
-            static const char* names[12] = {"prod.wait_aempty", "prod.total", "cons.wait_afull", "-", "cons.wait_wfull",
-                                            "-", "cons.wait_store", "-", "cons.wait_res", "-", "cons.total", "steps"};
-            fprintf(stderr, "[c3 prof] grid %d R %d n_mt %d nb %d N %d Cin %d w_res %d stg_bufs %d res %d steps %d:", q->grid, q->R, q->n_mt, q->nb,
-                    q->N, q->Cin, q->w_resident, q->stg_bufs, q->res != nullptr, q->total_steps);
-            for (int k = 0; k < 12; ++k) {
-                double acc = 0;
-                for (int c = 0; c < q->grid; ++c) acc += (double)h[(size_t)c * 16 + k];
-                fprintf(stderr, " %s=%.0f", names[k], acc / q->grid);
-            }
-            fprintf(stderr, "\n");
-            return nullptr;
-        };
-        return OpBuild::built;
-    }
     op->run = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
     return OpBuild::built;
 }
@@ -739,7 +681,7 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
 
 OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, const int* lens) {
     const int T = X.T, B = X.B;
-    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0 || getenv("WS_NO_CAM_FUSED"))
+    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0)
         return OpBuild::outside;
     auto q = std::make_shared<WsCamParams>();
     memset(q.get(), 0, sizeof(WsCamParams));
@@ -760,26 +702,6 @@ OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, i
     char buf[160];
     snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
     op->label = buf;
-    if (getenv("WS_CAM_PROF")) {   // tuning aid: synchronous launch + phase timestamps (cycles since kernel start) of CTA 0
-        long long* prof = nullptr;
-        if (cudaMalloc((void**)&prof, 16 * 8) != cudaSuccess) { set_err("cam_dense: prof buffer"); return OpBuild::error; }
-        cudaMemset(prof, 0, 16 * 8);
-        q->prof = prof;
-        op->run = [q](cudaStream_t s) -> const char* {
-            const char* m = ws_cam_launch(q.get(), s);
-            if (m) return m;
-            cudaStreamSynchronize(s);
-            long long h[16];
-            cudaMemcpy(h, q->prof, sizeof h, cudaMemcpyDeviceToHost);
-            static const char* names[12] = {"params", "transform_done", "acc1", "epi1", "colsums", "ctx", "hid_partial", "hid", "gate",
-                                            "acc2", "stored", "complete"};
-            fprintf(stderr, "[cam prof] B %d T %d l0 %d nst %d:", q->B, q->T, q->l0, q->nstages);
-            for (int k = 0; k < 12; ++k) fprintf(stderr, " %s=%lld", names[k], h[k]);
-            fprintf(stderr, "\n");
-            return nullptr;
-        };
-        return OpBuild::built;
-    }
     op->run = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
     return OpBuild::built;
 }
@@ -813,6 +735,7 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
     s.epi.bias = d->bias; s.epi.act1 = d->act1; s.epi.scale = d->scale; s.epi.shift = d->shift;
     s.epi.res = d->res; s.epi.res_ld = d->res_ld; s.epi.act2 = d->act2;
     s.epi.colsum = d->colsum; s.epi.colsum_T = d->colsum ? To : 0;
+    { const char* eg = getenv("WS_EPI_GENERIC"); s.epi_generic = eg != nullptr && atoi(eg) != 0; }
     PlanOp op;
     if (d->use_tc) { WS_CKS(ws_tc2_init()); WS_CKS(ws_tc3_init()); WS_CKS(ws_c3_init()); WS_CKS(ws_astp_init()); }
     bool done = false;

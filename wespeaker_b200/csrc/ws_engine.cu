@@ -91,7 +91,7 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
         e->plans.erase(victim);
     }
     p->last_use = ++e->use_clock;
-    p->lane = e->opt("plan_lanes", 1) ? (e->next_lane++ % ws_engine::kLanes) : 0;
+    p->lane = e->next_lane++ % ws_engine::kLanes;
     if (!e->plan_check && cudaEventCreateWithFlags(&p->done, cudaEventDisableTiming) != cudaSuccess) { set_err("plan event creation failed"); return nullptr; }
     Plan* raw = p.get();
     e->plans[key] = std::move(p);
@@ -349,8 +349,7 @@ int ws_engine_create_plan_check(const char* model_name, const char* precision, i
 int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
     if (!e || !key) { set_err("ws_engine_set_option: null argument"); return 1; }
     const std::string k = key;
-    if (k == "force_simt") { if (value) e->use_tc = 0; }
-    else if (k == "tc_version") {
+    if (k == "tc_version") {
         if (value != 2 && value != 3) {
             set_err("tc_version must be 2 (persistent tensor-core kernel) or 3 (+ weight-sharing clusters); 1, the one-tile-per-CTA "
                     "kernel, was removed");
@@ -363,7 +362,7 @@ int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
         e->sample_rate = (int)value;
         return 0;
     }
-    else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "plan_lanes" && k != "conv3x3_strided" && k != "astp_fused" && k != "plan_trace") { set_err("unknown option " + k); return 1; }
+    else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "astp_fused" && k != "plan_trace") { set_err("unknown option " + k); return 1; }
     e->opts[k] = value;
     e->plans.clear();
     return 0;

@@ -86,6 +86,7 @@ struct ConvSpec {
     int dt = WS_F32;
     WsEpi epi{};
     bool dense_pointwise = false;  // every tap has dt=df=0 on a dense src with the output's extents -> flatten positions
+    bool epi_generic = false;      // tensor-core kernels: run the generic epilogue even where the lean one applies (test reference)
 };
 
 // Append the taps of a (kf x kt) conv over `x` to `spec` (weights columns start at wk0, tap-major then channel).

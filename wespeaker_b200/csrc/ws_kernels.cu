@@ -908,7 +908,7 @@ const char* ws_launch_tstats(const void* x, int dt, int B, int F, int T, int C, 
         tmean8_kernel<<<g8, b8, 0, s>>>(x, dt, T, C, ld, (float*)out, out_ld);
         return last_err();
     }
-    if (dt != WS_F32 && C % 8 == 0 && ld % 8 == 0 && ((uintptr_t)x & 15) == 0 && !getenv("WS_TSTATS_SCALAR")) {
+    if (dt != WS_F32 && C % 8 == 0 && ld % 8 == 0 && ((uintptr_t)x & 15) == 0) {
         dim3 g8((C + 127) / 128, F, B), b8(16, 16);
         if (dt == WS_BF16) tstats8_kernel<WS_BF16><<<g8, b8, 0, s>>>(x, F, T, C, ld, pre_scale, pre_shift, out, odt, out_ld, std_off, eps, lens);
         else tstats8_kernel<WS_F16><<<g8, b8, 0, s>>>(x, F, T, C, ld, pre_scale, pre_shift, out, odt, out_ld, std_off, eps, lens);
@@ -970,8 +970,7 @@ const char* ws_launch_aff_combine(const void* x, long long x_ld, const void* y, 
 const char* ws_launch_astp_stats(const void* x, const void* logits, int dt, int B, int T, int C, long long ld,
                                  float* out, float var_floor, cudaStream_t s, const int* lens) {
     if (C % 2 != 0) return "astp_stats: C must be even";
-    static const int variant = getenv("WS_ASTP_VARIANT") ? atoi(getenv("WS_ASTP_VARIANT")) : 2;
-    if (variant == 2 && C % 4 == 0 && ld % 4 == 0 && dt != WS_F32 && T <= 256) {
+    if (C % 4 == 0 && ld % 4 == 0 && dt != WS_F32 && T <= 256) {
         dim3 grid((C + 63) / 64, B), block(16, 32);
         if (dt == WS_BF16) astp_stats4_kernel<WS_BF16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);
         else astp_stats4_kernel<WS_F16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);

@@ -398,15 +398,13 @@ struct Builder {
              tview("out", out) + "," + ti("C", C) + "}");
     }
     // The halo-resident 3x3 pad-1 conv (ws_conv3x3.cu: every input row crosses L2 -> SM once instead of once per tap),
-    // out = act(conv(x, W) + bias [+ res]).  halo3x3: whether the precision and the options let convs of strides (sf, st) use
-    // it.  halo_conv3x3 returns 1 with *op built (not pushed), 0 when the caller runs the conv-GEMM instead (also when the
-    // shape is outside the kernel's envelope), -1 on error.  lvl: stride level of `out`.
-    bool halo3x3(int sf, int st) const {
-        return e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("conv3x3", 1) != 0 && ((sf == 1 && st == 1) || e.opt("conv3x3_strided", 1) != 0);
-    }
+    // out = act(conv(x, W) + bias [+ res]).  halo3x3: whether the precision and the options let convs use it.  halo_conv3x3
+    // returns 1 with *op built (not pushed), 0 when the caller runs the conv-GEMM instead (also when the shape is outside
+    // the kernel's envelope), -1 on error.  lvl: stride level of `out`.
+    bool halo3x3() const { return e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("conv3x3", 1) != 0; }
     int halo_conv3x3(const View& x, const View& out, const void* W, const float* bias, const View* res, int act, int sf, int st, int lvl,
                      PlanOp* op) {
-        if (!halo3x3(sf, st)) return 0;
+        if (!halo3x3()) return 0;
         const OpBuild r = make_conv3x3_op(x, out, W, bias, res, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, op, sf, st, lens(lvl));
         if (r == OpBuild::error) ok = false;
         return r == OpBuild::built ? 1 : r == OpBuild::outside ? 0 : -1;
