@@ -66,27 +66,22 @@ def op_branches(op):
         out.add(f"astp_fused:chunks={min(n, 3)}")
         if n > 1 and T % 256 == 1:
             out.add("astp_fused:tail=1")
-    elif kind == "astp_stats":  # ws_launch_astp_stats (ws_kernels.cu:973)
-        x = tr["x"]
-        four = x["C"] % 4 == 0 and x["ld"] % 4 == 0 and tr["es"] == 2 and x["T"] <= 256
-        out.add("astp_stats:" + ("stats4" if four else "scalar"))
+    elif kind == "astp_stats":  # the kernel the plan chose (ws_astp_stats_kernel)
+        out.add("astp_stats:" + tr["kernel"])
     elif kind == "se_gate":     # two utterances per CTA
         if tr["x"]["B"] % 2:
             out.add("se_gate:odd-B")
         if tr["x"]["T"] < 128:
             out.add("se_gate:T<128")
-    elif kind == "tstats":      # ws_launch_tstats (ws_kernels.cu:905-917)
-        x = tr["x"]
-        if tr["std_off"] < 0 and x["F"] == 1 and not tr["pre_scale"] and x["C"] % 8 == 0 and not masked:
-            out.add("tmean8")
-        elif tr["es"] == 2 and x["C"] % 8 == 0 and x["ld"] % 8 == 0:
-            T = x["T"]      # tstats8's 4-wide loop runs while t + 48 < T, t = slice (0..15) + 64 k
+    elif kind == "tstats":      # the kernel the plan chose (ws_tstats_kernel)
+        k = tr["kernel"]
+        if k == "tstats8":
+            T = tr["x"]["T"]    # tstats8's 4-wide loop runs while t + 48 < T, t = slice (0..15) + 64 k
             out.add("tstats8:" + ("T<=48" if T <= 48 else "49<=T<64" if T < 64 else "T>=64"))
         else:
-            out.add("tstats:scalar")
-    elif kind == "linear":      # ws_linear_rows_big (ws_kernels.cu:922); split-K when the launch would not fill the SMs
-        big = tr["R"] >= 48 and tr["O"] >= 48 and tr["I"] % 4 == 0 and tr["in_ld"] % 4 == 0 and (not tr["in2"] or tr["in2_ld"] % 4 == 0)
-        out.add("linear:" + ("rows64" if big else "rows16"))
+            out.add("tmean8" if k == "tmean8" else "tstats:" + k)
+    elif kind == "linear":      # the kernel the plan chose (ws_linear_rows_plan); split-K when the launch would not fill the SMs
+        out.add("linear:" + tr["kernel"])
         if tr.get("wsp"):
             out.add("linear:split-K")
     elif kind == "stem":        # 128-frame tiles

@@ -267,7 +267,7 @@ def run_tstats(mem, tr):
         xe = np.abs(x * mem.vec(tr["pre_scale"], C)) + np.abs(mem.vec(tr["pre_shift"], C))
         x = np.maximum(x * mem.vec(tr["pre_scale"], C) + mem.vec(tr["pre_shift"], C), 0.0)
     out_ld, so = tr["out_ld"], tr["std_off"]
-    out = mem.strided(tr["out"], 4, (B, out_ld), (out_ld, 1), write=True)
+    out = mem.strided(tr["out"], tr["out_es"], (B, out_ld), (out_ld, 1), write=True)
     lens = mem.vec(tr["lens"], B).astype(int) if tr["lens"] else np.full(B, T)   # statistics over each utterance's own frames
     err = np.zeros((B, out_ld))
     for b in range(B):
@@ -277,7 +277,7 @@ def run_tstats(mem, tr):
         eb = xe[b, :, :n]
         err[b, :C * F] = (n * np.abs(xb).mean(axis=1) + eb.mean(axis=1)).T.reshape(C * F)   # a sum of n terms: gamma_n
         if so >= 0:
-            sd = np.sqrt(xb.var(axis=1, ddof=1) + 1e-7)
+            sd = np.sqrt(xb.var(axis=1, ddof=1) + tr["eps"])
             out[b, so:so + C * F] = sd.T.reshape(C * F)
             # var error <= n u (sum x^2) / (n - 1) whether it is summed in one pass or two; d(std) = d(var) / (2 std)
             dvar = (n * (xb * xb).sum(axis=1) + 2 * (np.abs(xb - xb.mean(axis=1, keepdims=True)) * eb).sum(axis=1)) / max(n - 1, 1)
@@ -364,9 +364,14 @@ def run_res2_fused(mem, tr):
 
 
 def run_se_gate(mem, tr):
-    """gate[b][c] = sigmoid(W2 relu(W1 mean_T(x[b]) + b1) + b2); W2t is W2 transposed to [H][C] (ecapa_tdnn.py:113-126)."""
+    """gate[b][c] = sigmoid(W2 relu(W1 mean_T(x[b]) + b1) + b2); W2t is W2 transposed to [H][C] (ecapa_tdnn.py:113-126).
+    With colsum, the kernel sums the column sums the producing conv's epilogue wrote instead of reading x; the contract is
+    still the mean of x."""
     x = mem.view(tr["x"], tr["es"])[:, 0]
     B, T, C = x.shape
+    if tr["colsum"]:    # the rest of the column-sum buffer
+        base, nbytes = mem._find(tr["colsum"])
+        mem.read(tr["colsum"], 4, ((base + nbytes - tr["colsum"]) // 4,), (1,))
     H = tr["H"]
     W1 = mem.vec(tr["W1"], H * C).reshape(H, C)
     W2t = mem.vec(tr["W2t"], H * C).reshape(H, C)

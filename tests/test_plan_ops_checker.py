@@ -333,3 +333,18 @@ def test_unwritten_one_row_time_tile_is_flagged():
         bad[base].numpy()[s:s + n] = state[base].numpy()[s:s + n]
     assert not pi.check_op(meta, meta["ops"][i], state, good)[1]
     flagged(meta, i, state, bad)
+
+
+def test_se_gate_reads_the_column_sums_its_conv_wrote():
+    """A 16-bit ECAPA plan at T >= 128 squeezes SE from the column sums the preceding conv's epilogue writes: the se_gate
+    trace names that buffer, and its contract declares the read."""
+    meta, blob = trace_of("ECAPA_TDNN_c512", "bf16", 2, 200)
+    ops = [op["trace"] for op in meta["ops"]]
+    gates = [i for i, tr in enumerate(ops) if tr["kind"] == "se_gate"]
+    assert gates
+    for i in gates:
+        conv = next(tr for tr in reversed(ops[:i]) if tr["kind"] == "conv")
+        assert conv["colsum"] and ops[i]["colsum"] == conv["colsum"]
+        mem = pi.Memory(meta, blob)
+        pi.run_op(mem, ops[i], meta)
+        assert any(addr == conv["colsum"] for addr, *_ in mem.reads)

@@ -11,9 +11,10 @@ the plan builders leaves the plans alone:
 The trace's placeholder addresses depend on what was allocated before, so each one is written in canonical form: an
 activation address becomes "A<k>+<offset>" with allocations numbered in order of first reference (header, then ops), and a
 weight address becomes "W<sha256 of its fp32 source>+<offset>".  --out DIR also writes each case's canonical plan to
-DIR/<case>.json, for diffing the cases whose digests differ.  --strip-added drops the optional buffer fields (the 3xTF32
-lo twins plo, p_lo, W_lo, out_lo, out2_lo, the linear split-K workspace wsp and the SimAM partial sums) before digesting, for comparing with builds
-whose traces did not name them.
+DIR/<case>.json, for diffing the cases whose digests differ.  --strip-added drops the fields that later traces added before
+digesting, for comparing with builds whose traces did not name them: the optional buffers (the 3xTF32 lo twins plo, p_lo,
+W_lo, out_lo, out2_lo, the linear split-K workspace wsp and the SimAM partial sums), the kernel an op takes, tstats' eps and
+output element size, and se_gate's column sums ("kind.field": that field of that op kind only).
 """
 import argparse
 import bisect
@@ -33,7 +34,8 @@ from wespeaker_b200.models import SUPPORTED_MODELS, from_synthetic  # noqa: E402
 
 PRECISIONS = ("fp32", "tf32", "tf32x3", "bf16", "fp16")
 PLACEHOLDER = 0x7000000000   # plan_check_alloc hands out addresses from here up
-ADDED_FIELDS = ("plo", "p_lo", "W_lo", "out_lo", "out2_lo", "wsp", "partial")
+ADDED_FIELDS = ("plo", "p_lo", "W_lo", "out_lo", "out2_lo", "wsp", "partial", "kernel", "tstats.eps", "tstats.out_es",
+                "se_gate.colsum")
 
 
 def cases():
@@ -74,7 +76,8 @@ def case_id(c):
 
 def _strip_added(x):
     if isinstance(x, dict):
-        return {k: _strip_added(v) for k, v in x.items() if k not in ADDED_FIELDS}
+        kind = x.get("kind")
+        return {k: _strip_added(v) for k, v in x.items() if k not in ADDED_FIELDS and f"{kind}.{k}" not in ADDED_FIELDS}
     if isinstance(x, list):
         return [_strip_added(v) for v in x]
     return x

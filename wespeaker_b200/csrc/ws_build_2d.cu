@@ -110,15 +110,7 @@ View stem(Builder& b, const std::string& convkey, const std::string& bnkey, View
     const int B = b.p.B, T = b.p.T, Fd = b.e.feat_dim;
     const View o = outbuf.shaped(B, Fd, T, co);
     const float* wd = b.w.f32("w:" + convkey + ".stem", w9);   // [Cout][9] (tap = df*3 + dt)
-    const float* hd = b.w.f32("bnh:" + bnkey, h);
-    const float* fin = b.p.feats_in;
-    const int dt = b.e.act_dt;
-    void* op = o.p;
-    float* olo = (float*)o.plo;
-    const int* l0 = b.lens(0);
-    b.push([=](cudaStream_t st) { return ws_launch_stem(fin, wd, hd, op, olo, dt, B, T, Fd, co, st, l0); }, "stem",
-           "{\"kind\":\"stem\"," + ti("es", ws_esize(dt)) + "," + tp("feats", fin) + "," + tp("w9", wd) + "," + tp("shift", hd) + "," +
-           tview("out", o) + "," + ti("Fdim", Fd) + "," + tp("lens", l0) + "}");
+    b.push(WsStem{b.p.feats_in, wd, b.w.f32("bnh:" + bnkey, h), o, b.lens(0)}, ws_launch_stem, "stem");
     return o;
 }
 
@@ -263,13 +255,7 @@ static bool aff(Builder& b, const std::string& p, const View& x, const View& y, 
     eb.act1 = WS_ACT_TANH;
     b.conv_simple(hid, att, b.w.act("w:" + p + ".att3", wbp), 1, 1, 1, 1, 0, 0, 1, 1, eb);
     if (!b.good()) return false;
-    const View xv = x, yv = y, av = att, ov = out;
-    const int dt = b.e.act_dt;
-    const long long npos = x.npos();
-    b.push([=](cudaStream_t s) {
-        return ws_launch_aff_combine(xv.p, xv.ld, yv.p, yv.ld, av.p, av.ld, ov.p, (float*)ov.plo, ov.ld, dt, npos, Cp, s);
-    }, "aff_combine", "{\"kind\":\"aff_combine\"," + ti("es", ws_esize(dt)) + "," + tview("x", xv) + "," + tview("y", yv) + "," + tview("t", av) + "," +
-                      tview("out", ov) + "}");
+    b.push(WsAffCombine{x, y, att, out}, ws_launch_aff_combine, "aff_combine");
     return b.good();
 }
 
@@ -465,20 +451,11 @@ constexpr float kSimamLambda = 1e-4f;   // samresnet.py:65
 
 // out = relu(SimAM(y) + res), out at element b*os.b + f*os.f + t*os.t + c (y's extents); lvl: stride level of y
 static bool simam(Builder& b, const View& y, const View& res, const View& out, WsMapStrides os, float* partial, float* stats, int lvl) {
-    const View yv = y, rv = res;
-    void* op_ = out.p;
-    float* olo = (float*)out.plo;
     const WsMapStrides rs{(long long)res.F * res.T * res.ld, (long long)res.T * res.ld, res.ld};
     const int* l = b.lens(lvl);
-    const int dt = b.e.act_dt;
-    b.push([=](cudaStream_t s) { return ws_launch_simam_stats(yv.p, dt, yv.B, yv.F, yv.T, yv.C, yv.ld, partial, stats, s, l); }, "simam_stats",
-           "{\"kind\":\"simam_stats\"," + ti("es", ws_esize(dt)) + "," + tview("x", yv) + "," + tp("stats", stats) + "," + tp("lens", l) + tplo("partial", partial) + "}");
+    b.push(WsSimamStats{y, partial, stats, l}, ws_launch_simam_stats, "simam_stats");
     b.p.extra_launches += 1;   // partials + merge
-    b.push([=](cudaStream_t s) {
-        return ws_launch_simam_apply(yv.p, yv.ld, stats, kSimamLambda, rv.p, rs, op_, olo, os, dt, yv.B, yv.F, yv.T, yv.C, s, l);
-    }, "simam_apply", "{\"kind\":\"simam_apply\"," + ti("es", ws_esize(dt)) + "," + tview("y", yv) + "," + tp("stats", stats) + "," +
-                      tview("res", rv) + "," + tp("out", op_) + "," + ti("out_sb", os.b) + "," + ti("out_sf", os.f) + "," +
-                      ti("out_st", os.t) + "," + tp("lens", l) + ",\"lambda\":1e-4}");
+    b.push(WsSimamApply{y, stats, kSimamLambda, res.p, rs, out.p, (float*)out.plo, os, l}, ws_launch_simam_apply, "simam_apply");
     return b.good();
 }
 
@@ -604,12 +581,7 @@ static bool dwconv3x3(Builder& b, const std::string& id, const View& x, const Vi
         b.ok = false;
         return false;
     }
-    const View xv = x, ov = out;
-    const int* l = b.lens(lvl);
-    b.push([=](cudaStream_t s) {
-        return ws_launch_dwconv3x3(xv.p, xv.ld, w9, shift, ov.p, (float*)ov.plo, ov.ld, xv.dt, xv.B, xv.F, xv.T, xv.C, s, l);
-    }, "dwconv3x3", "{\"kind\":\"dwconv3x3\"," + ti("es", ws_esize(xv.dt)) + "," + tview("x", xv) + "," + tview("out", ov) + "," +
-                    tp("w", w9) + "," + tp("shift", shift) + "," + tp("lens", l) + "}");
+    b.push(WsDwconv3x3{x, w9, shift, out, b.lens(lvl)}, ws_launch_dwconv3x3, "dwconv3x3");
     return b.good();
 }
 

@@ -116,22 +116,17 @@ bool build_ecapa(Builder& b) {
         }
         // SE_Connect (ecapa_tdnn.py:113-126) + residual (:157)
         if (e.opt("se_fused", 1) && (C == 512 || C == 1024)) {
-            const HostT* w2 = b.w.get(pf + ".3.linear2.weight");   // (C, 128) -> transposed (128, C) for coalesced reads
+            const int H = 128;   // SE bottleneck width
+            const HostT* w2 = b.w.get(pf + ".3.linear2.weight");   // (C, H) -> transposed (H, C) for coalesced reads
             if (!w2) break;
-            std::vector<float> w2t((size_t)128 * C);
+            std::vector<float> w2t((size_t)H * C);
             for (int c = 0; c < C; ++c)
-                for (int h = 0; h < 128; ++h) w2t[(size_t)h * C + c] = w2->v[(size_t)c * 128 + h];
+                for (int h = 0; h < H; ++h) w2t[(size_t)h * C + c] = w2->v[(size_t)c * H + h];
             const float* w1d = b.w.vec(pf + ".3.linear1.weight");
             const float* b1d = b.w.vec(pf + ".3.linear1.bias");
             const float* w2d = b.w.f32("w2t:" + pf, w2t);
             const float* b2d = b.w.vec(pf + ".3.linear2.bias");
-            View tc = tC;
-            const int dt = e.act_dt;
-            const float* cs_in = se_colsum;
-            const int* l0 = b.lens(0);
-            b.push([=](cudaStream_t s) { return ws_launch_se_gate(tc.p, dt, B, T, C, tc.ld, w1d, b1d, w2d, b2d, 128, segate, cs_in, s, l0); }, "se_gate",
-                   "{\"kind\":\"se_gate\"," + ti("es", ws_esize(dt)) + "," + tview("x", tc) + "," + tp("W1", w1d) + "," + tp("b1", b1d) + "," +
-                   tp("W2t", w2d) + "," + tp("b2", b2d) + "," + ti("H", 128) + "," + tp("gate", segate) + "," + tp("lens", l0) + "}");
+            b.push(WsSeGate{tC, w1d, b1d, w2d, b2d, H, segate, se_colsum, b.lens(0)}, ws_launch_se_gate, "se_gate");
         } else {
             b.tstats(tC, nullptr, nullptr, semean, C, -1);
             b.linear(semean, C, nullptr, 0, 1, b.w.vec(pf + ".3.linear1.weight"), b.w.vec(pf + ".3.linear1.bias"), sehid, 128, B,
@@ -140,12 +135,8 @@ bool build_ecapa(Builder& b) {
                      B, 128, C, WS_ACT_SIGMOID);
         }
         {
-            View o = cat.ch((L - 2) * C, C), xi = xin, tc = tC;
-            const int dt = e.act_dt;
-            b.push([=](cudaStream_t s) {
-                return ws_launch_scale_residual(tc.p, tc.ld, segate, xi.p, xi.ld, o.p, (float*)o.plo, o.ld, dt, B, T, C, s);
-            }, "scale_residual", "{\"kind\":\"scale_residual\"," + ti("es", ws_esize(dt)) + "," + tview("x", tc) + "," + tp("gate", segate) + "," +
-                                 tview("res", xi) + "," + tview("out", o) + "}");
+            const View o = cat.ch((L - 2) * C, C);
+            b.push(WsScaleResidual{tC, segate, xin, o}, ws_launch_scale_residual, "scale_residual");
             xin = o;
         }
     }

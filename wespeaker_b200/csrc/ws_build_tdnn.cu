@@ -85,7 +85,7 @@ bool build_campplus(Builder& b) {
     View Xf = b.act(B, 1, Tp, cmax[2] / 2);
     View scratch = b.act(B, 1, Tp, cmax[2]);
     View hid = b.act(B, 1, Tp, bnc);
-    const int nseg = (Tp + 99) / 100;
+    const int nseg = (Tp + kCamSegLen - 1) / kCamSegLen;
     float* cmean = b.f32((size_t)B * bnc);
     float* csegm = b.f32((size_t)B * nseg * bnc);
     float* chid = b.f32((size_t)B * nseg * (bnc / 2));
@@ -126,14 +126,13 @@ bool build_campplus(Builder& b) {
         fill_epi_out(cs.epi, X[0].ch(0, co));
         b.conv(cs);
     }
-    const int dt = e.act_dt;
     // Fused dense layers (ws_cam_dense.cu): one launch per CAMDenseTDNNLayer (or per block with cam_block = 1) instead of four
     const bool cam_fused = e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("cam_fused", 1) != 0 && Tp <= 512;
     for (int bl = 0; bl < 3 && b.good(); ++bl) {
         bool fused_done = false;
         if (cam_fused) {
             std::vector<WsCamLayer> hl((size_t)nl[bl]);
-            std::vector<std::string> hl_trace((size_t)nl[bl]);   // plan-check engines: what each layer descriptor points at
+            std::vector<std::array<const void*, 2>> hw((size_t)nl[bl]);   // the (W1, Wl) each descriptor's tensor maps encode
             bool okl = true;
             for (int j = 1; j <= nl[bl] && okl; ++j) {
                 const std::string p = "xvector.block" + std::to_string(bl + 1) + ".tdnnd" + std::to_string(j);
@@ -159,10 +158,7 @@ bool build_campplus(Builder& b) {
                 const float* w2cd = b.w.f32("w2ct:" + p, w2ct);
                 const float* b2cd = b.w.vec(p + ".cam_layer.linear2.bias");
                 okl = cam_layer_fill(&hl[(size_t)j - 1], e.act_dt, W1d, Wld, s1d, h1d, h2d, w1cd, b1cd, w2cd, b2cd, cin, dil[bl]);
-                if (plan_trace_mode())
-                    hl_trace[(size_t)j - 1] = "{" + tp("W1", W1d) + "," + tp("Wl", Wld) + "," + tp("bn1_scale", s1d) + "," + tp("bn1_shift", h1d) +
-                                              "," + tp("bias2", h2d) + "," + tp("w1c_t", w1cd) + "," + tp("b1c", b1cd) + "," + tp("w2c_t", w2cd) + "," +
-                                              tp("b2c", b2cd) + "," + ti("cin", cin) + "," + ti("dil", dil[bl]) + "}";
+                hw[(size_t)j - 1] = {W1d, Wld};
             }
             if (!okl || !b.good()) { b.ok = false; break; }
             const WsCamLayer* ldev = (const WsCamLayer*)b.w.upload("camlayers:" + std::to_string(bl), hl.data(), hl.size() * sizeof(WsCamLayer));
@@ -172,16 +168,8 @@ bool build_campplus(Builder& b) {
             for (int j = 0; j < nl[bl]; j += whole ? nl[bl] : 1) {
                 const int j1 = whole ? nl[bl] : j + 1;
                 PlanOp op;
-                const OpBuild r = make_cam_dense_op(X[bl], ldev, j, j1, &op, b.lens(1));
-                if (r == OpBuild::built) {
-                    if (plan_trace_mode()) {   // semantic description of the fused launch: layers [j, j1) over the concat buffer
-                        op.trace = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(e.act_dt)) + "," + tview("X", X[bl]) + "," + tp("lens", b.lens(1)) + "," +
-                                   ti("seg_len", 100) + ",\"layers\":[";
-                        for (int k = j; k < j1; ++k) op.trace += std::string(k > j ? "," : "") + hl_trace[(size_t)k];
-                        op.trace += "]}";
-                    }
-                    b.push(std::move(op));
-                }
+                const OpBuild r = make_cam_dense_op(X[bl], ldev, hl, hw, j, j1, &op, b.lens(1));
+                if (r == OpBuild::built) b.push(std::move(op));
                 else if (r == OpBuild::outside && j == 0) { fused_done = false; break; }
                 else { b.ok = false; break; }
             }
@@ -197,14 +185,13 @@ bool build_campplus(Builder& b) {
                 break;
             // nonlinear1 (BN-ReLU on the growing concat) -> scratch
             const View sv = scratch.shaped(B, 1, Tp, cin);
-            b.bnrelu(X[bl].ch(0, cin), b.w.f32("bns:" + p + ".n1", s1), b.w.f32("bnh:" + p + ".n1", h1), sv);
+            b.push(WsBnRelu{X[bl].ch(0, cin), b.w.f32("bns:" + p + ".n1", s1), b.w.f32("bnh:" + p + ".n1", h1), sv}, ws_launch_bnrelu, "bnrelu");
             // linear1 (1x1, no bias) + nonlinear2 (BN folded) + ReLU -> hid
             WsEpi e1{};
             e1.bias = b.w.f32("bnh:" + p + ".n2", h2);
             e1.act1 = WS_ACT_RELU;
             b.conv_simple(sv, hid, b.w.act("w:" + p + ".linear1", w1), 1, 1, 1, 1, 0, 0, 1, 1, e1);
             // CAM context mask (campplus.py:108-115): sigmoid(W2 relu(W1 (mean_T + segmean_100)))
-            View hv = hid;
             {
                 const float* w1c = b.w.vec(p + ".cam_layer.linear1.weight");
                 const float* b1c = b.w.vec(p + ".cam_layer.linear1.bias");
@@ -212,22 +199,16 @@ bool build_campplus(Builder& b) {
                 const float* b2c = b.w.vec(p + ".cam_layer.linear2.bias");
                 const size_t cam_smem = (size_t)((bnc / 2) * bnc + nseg * bnc + 16 * bnc + nseg * (bnc / 2) + bnc) * 4;
                 if (cam_smem <= 48 * 1024) {
-                    b.push([=](cudaStream_t st) {
-                        return ws_launch_cam_gate(hv.p, dt, B, Tp, bnc, hv.ld, 100, w1c, b1c, w2c, b2c, bnc / 2, growth, cgate, st);
-                    }, "cam_gate", "{\"kind\":\"cam_gate\"," + ti("es", ws_esize(dt)) + "," + tview("x", hv) + "," + ti("seg_len", 100) + "," + tp("W1", w1c) + "," +
-                                   tp("b1", b1c) + "," + tp("W2", w2c) + "," + tp("b2", b2c) + "," + ti("H", bnc / 2) + "," + ti("G", growth) + "," +
-                                   tp("gate", cgate) + "}");
+                    b.push(WsCamGate{hid, kCamSegLen, w1c, b1c, w2c, b2c, bnc / 2, growth, cgate}, ws_launch_cam_gate, "cam_gate");
                 } else {  // very long utterances: unfused path
-                    b.push([=](cudaStream_t st) { return ws_launch_seg_means(hv.p, dt, B, Tp, bnc, hv.ld, 100, cmean, csegm, st); }, "seg_means",
-                           "{\"kind\":\"seg_means\"," + ti("es", ws_esize(dt)) + "," + tview("x", hv) + "," + ti("seg_len", 100) + "," + tp("mean", cmean) + "," +
-                           tp("segmean", csegm) + "}");
+                    b.push(WsSegMeans{hid, kCamSegLen, cmean, csegm}, ws_launch_seg_means, "seg_means");
                     b.linear(csegm, bnc, cmean, bnc, nseg, w1c, b1c, chid, bnc / 2, B * nseg, bnc, bnc / 2, WS_ACT_RELU);
                     b.linear(chid, bnc / 2, nullptr, 0, 1, w2c, b2c, cgate, growth, B * nseg, bnc / 2, growth, WS_ACT_SIGMOID);
                 }
             }
             // linear_local (k3, dilated, no bias) * mask -> appended to the concat buffer
             WsEpi e2{};
-            e2.gate = cgate; e2.gate_ld = growth; e2.gate_seg = 100; e2.gate_nseg = nseg;
+            e2.gate = cgate; e2.gate_ld = growth; e2.gate_seg = kCamSegLen; e2.gate_nseg = nseg;
             b.conv_simple(hid, X[bl].ch(cin, growth), b.w.act("w:" + p + ".local", wl), 1, 3, 1, dil[bl], 0, dil[bl], 1, 1, e2);
         }
         if (!b.good()) break;
@@ -236,7 +217,7 @@ bool build_campplus(Builder& b) {
         std::vector<float> s, h, wt;
         if (!b.w.bn(tk + ".nonlinear.batchnorm", true, s, h) || !b.w.pack_conv(tk + ".linear.weight", nullptr, wt)) break;
         const View sv = scratch.shaped(B, 1, Tp, cmax[bl]);
-        b.bnrelu(X[bl], b.w.f32("bns:" + tk, s), b.w.f32("bnh:" + tk, h), sv);
+        b.push(WsBnRelu{X[bl], b.w.f32("bns:" + tk, s), b.w.f32("bnh:" + tk, h), sv}, ws_launch_bnrelu, "bnrelu");
         WsEpi et{};
         View dst = (bl < 2) ? X[bl + 1].ch(0, cmax[bl] / 2) : Xf;
         b.conv_simple(sv, dst, b.w.act("w:" + tk, wt), 1, 1, 1, 1, 0, 0, 1, 1, et);

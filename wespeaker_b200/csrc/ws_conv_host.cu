@@ -21,10 +21,6 @@ static thread_local bool g_plan_check = false;
 bool plan_check_mode() { return g_plan_check; }
 PlanCheckScope::PlanCheckScope(bool on) : prev(g_plan_check) { g_plan_check = on; }
 PlanCheckScope::~PlanCheckScope() { g_plan_check = prev; }
-static thread_local bool g_plan_trace = false;
-bool plan_trace_mode() { return g_plan_trace; }
-PlanTraceScope::PlanTraceScope(bool on) : prev(g_plan_trace) { g_plan_trace = on; }
-PlanTraceScope::~PlanTraceScope() { g_plan_trace = prev; }
 static std::string conv_trace(const ConvSpec& s) {
     std::string j = "{\"kind\":\"conv\"," + ti("es", ws_esize(s.dt)) + ",\"src\":[";
     for (int i = 0; i < s.nsrc; ++i) {
@@ -389,7 +385,7 @@ static void label_conv(PlanOp* op, const char* kern, const ConvSpec& spec) {
     op->flops = 2.0 * pos * spec.Ktot * spec.Cout;
 }
 bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
-    if (plan_trace_mode()) out->trace = conv_trace(spec);
+    out->trace = [spec] { return conv_trace(spec); };
     const char* env_mp = getenv("WS_TC3_MIN_POS");
     const long long min_pos = env_mp ? atoll(env_mp) : 132LL * 128;   // one wave of 128-row tiles on an H100
     if (use_tc >= 3 && (long long)spec.B * spec.F * spec.T >= min_pos) {
@@ -457,9 +453,8 @@ OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float
     const long long units = (long long)x.B * q->ntile;
     q->grid = (int)(units < ws_num_sms() ? units : ws_num_sms());
     op->run = [q](cudaStream_t s) { return ws_res2_launch(q.get(), s); };
-    if (plan_trace_mode())
-        op->trace = "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W7", W7) + "," + tp("bias", bias) +
-                    "," + tp("scale", scale) + "," + tp("shift", shift) + "," + ti("w8", w8) + "," + ti("dil", dil) + "," + tp("lens", lens) + "}";
+    op->trace = [=] { return "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W7", W7) + "," + tp("bias", bias) + "," +
+               tp("scale", scale) + "," + tp("shift", shift) + "," + ti("w8", w8) + "," + ti("dil", dil) + "," + tp("lens", lens) + "}"; };
     char buf[160];
     snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", x.B, x.T, x.C);
     op->label = buf;
@@ -508,9 +503,8 @@ OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats,
     const long long units = (long long)x.B * (nblk / q->g);
     q->grid = (int)(units < sms ? units : sms);
     op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
-    if (plan_trace_mode())
-        op->trace = "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) +
-                    "," + tp("lens", lens) + "," + tf("eps", var_floor) + "}";
+    op->trace = [=] { return "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) + "," +
+               tp("lens", lens) + "," + tf("eps", var_floor) + "}"; };
     char buf[160];
     snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);
     op->label = buf;
@@ -646,10 +640,10 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
              q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
     op->label = buf;
     op->flops = 2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout;
-    if (plan_trace_mode())
-        op->trace = "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) +
-                    "," + (res ? tview("res", *res) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) +
-                    "," + tp("lens", lens) + "}";
+    const bool has_res = res != nullptr;
+    const View rv = has_res ? *res : View();
+    op->trace = [=] { return "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) + "," +
+               (has_res ? tview("res", rv) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) + "," + tp("lens", lens) + "}"; };
     op->run = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
     return OpBuild::built;
 }
@@ -679,14 +673,15 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
     return true;
 }
 
-OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, const int* lens) {
+OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std::vector<WsCamLayer>& layers,
+                          const std::vector<std::array<const void*, 2>>& weights, int l0, int l1, PlanOp* op, const int* lens) {
     const int T = X.T, B = X.B;
     if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0)
         return OpBuild::outside;
     auto q = std::make_shared<WsCamParams>();
     memset(q.get(), 0, sizeof(WsCamParams));
     q->layers = layers_dev; q->l0 = l0; q->l1 = l1; q->lens = lens;
-    q->B = B; q->T = T; q->nmt = (T + 127) / 128; q->seg_len = 100; q->dtype = X.dt;
+    q->B = B; q->T = T; q->nmt = (T + 127) / 128; q->seg_len = kCamSegLen; q->dtype = X.dt;
     q->hrows = 16 + 128 * q->nmt;
     int nst = 6;
     while (nst >= 2 && ws_cam_smem_bytes(q->nmt, nst) > ws_cam_max_smem()) --nst;
@@ -703,6 +698,20 @@ OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, i
     snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
     op->label = buf;
     op->run = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
+    // layers [l0, l1) over the concat buffer, each with what its descriptor points at
+    const std::vector<WsCamLayer> ls(layers.begin() + l0, layers.begin() + l1);
+    const std::vector<std::array<const void*, 2>> lw(weights.begin() + l0, weights.begin() + l1);
+    op->trace = [=] {
+        std::string j = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(X.dt)) + "," + tview("X", X) + "," + tp("lens", lens) + "," +
+                         ti("seg_len", q->seg_len) + ",\"layers\":[";
+        for (size_t k = 0; k < ls.size(); ++k) {
+            const WsCamLayer& L = ls[k];
+            j += std::string(k ? "," : "") + "{" + tp("W1", lw[k][0]) + "," + tp("Wl", lw[k][1]) + "," + tp("bn1_scale", L.bn1_scale) + "," +
+                 tp("bn1_shift", L.bn1_shift) + "," + tp("bias2", L.bias2) + "," + tp("w1c_t", L.w1c_t) + "," + tp("b1c", L.b1c) + "," +
+                 tp("w2c_t", L.w2c_t) + "," + tp("b2c", L.b2c) + "," + ti("cin", L.cin) + "," + ti("dil", L.dil) + "}";
+        }
+        return j + "]}";
+    };
     return OpBuild::built;
 }
 

@@ -136,8 +136,12 @@ bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace
 
-const char* ws_launch_dwconv3x3(const void* x, long long x_ld, const float* w, const float* shift, void* out, float* out_lo,
-                                long long out_ld, int dt, int B, int F, int T, int C, cudaStream_t s, const int* lens) {
+const char* ws_launch_dwconv3x3(const WsDwconv3x3& a, cudaStream_t s) {
+    const void *x = a.x.p, *w = a.w, *shift = a.shift;
+    void* out = a.out.p;
+    float* out_lo = (float*)a.out.plo;
+    const long long x_ld = a.x.ld, out_ld = a.out.ld;
+    const int dt = a.x.dt, B = a.x.B, F = a.x.F, T = a.x.T, C = a.x.C;
     if (dt != WS_F32 && dt != WS_BF16 && dt != WS_F16) return "dwconv3x3: dtype must be 0 (fp32), 1 (bf16) or 2 (fp16)";
     const int V = 16 / ws_esize(dt);   // channels per 16-byte copy
     if (C % V != 0 || x_ld % V != 0 || out_ld % V != 0 || x_ld < C || out_ld < C || !aligned16(x) || !aligned16(out) || !aligned16(w) ||
@@ -161,17 +165,18 @@ const char* ws_launch_dwconv3x3(const void* x, long long x_ld, const float* w, c
     const dim3 grid(nchunk * ntile, nband, B);
     const int smem = (fb + 2) * (tt + 2) * kCh * ws_esize(dt);
     if (dt == WS_BF16)
-        dwconv3x3_kernel<WS_BF16><<<grid, kThreads, smem, s>>>(x, x_ld, w, shift, out, nullptr, out_ld, F, T, C, fb, tt, nchunk, lens);
+        dwconv3x3_kernel<WS_BF16><<<grid, kThreads, smem, s>>>(x, x_ld, a.w, a.shift, out, nullptr, out_ld, F, T, C, fb, tt, nchunk, a.lens);
     else if (dt == WS_F16)
-        dwconv3x3_kernel<WS_F16><<<grid, kThreads, smem, s>>>(x, x_ld, w, shift, out, nullptr, out_ld, F, T, C, fb, tt, nchunk, lens);
+        dwconv3x3_kernel<WS_F16><<<grid, kThreads, smem, s>>>(x, x_ld, a.w, a.shift, out, nullptr, out_ld, F, T, C, fb, tt, nchunk, a.lens);
     else
-        dwconv3x3_kernel<WS_F32><<<grid, kThreads, smem, s>>>(x, x_ld, w, shift, out, out_lo, out_ld, F, T, C, fb, tt, nchunk, lens);
+        dwconv3x3_kernel<WS_F32><<<grid, kThreads, smem, s>>>(x, x_ld, a.w, a.shift, out, out_lo, out_ld, F, T, C, fb, tt, nchunk, a.lens);
     return last_err();
 }
 
 extern "C" int ws_dwconv(const ws_dwconv_desc* d, void* stream) {
     if (!d || !d->x || !d->w || !d->shift || !d->out) { ws::set_err("ws_dwconv: null argument"); return 1; }
-    WS_CKS(ws_launch_dwconv3x3(d->x, d->x_ld, d->w, d->shift, d->out, (float*)d->out_lo, d->out_ld, d->dtype, d->B, d->F, d->T, d->C,
-                               (cudaStream_t)stream, d->lens));
+    const WsView x{const_cast<void*>(d->x), nullptr, d->B, d->F, d->T, d->C, d->x_ld, d->dtype},
+        out{d->out, d->out_lo, d->B, d->F, d->T, d->C, d->out_ld, d->dtype};
+    WS_CKS(ws_launch_dwconv3x3(WsDwconv3x3{x, d->w, d->shift, out, d->lens}, (cudaStream_t)stream));
     return 0;
 }

@@ -64,15 +64,10 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
     std::unique_ptr<Plan> p(new Plan());
     p->B = B; p->T = T; p->masked = masked; p->check = e->plan_check;
     PlanCheckScope check_scope(e->plan_check);
-    PlanTraceScope trace_scope(e->plan_check || e->opt("plan_trace", 0) != 0);
     Builder b(*e, *p);
     if (masked) {
         p->lens = (int*)b.raw((size_t)4 * B * sizeof(int));
-        int* l = p->lens;
-        if (b.good()) {
-            b.push([=](cudaStream_t s) { return ws_launch_lens_derive(l, B, T, 4, s); }, "lens_derive",
-                   "{\"kind\":\"lens_derive\"," + tp("lens", l) + "," + ti("B", B) + "," + ti("T", T) + "," + ti("levels", 4) + "}");
-        }
+        if (b.good()) b.push(WsLensDerive{p->lens, B, T, 4}, ws_launch_lens_derive, "lens_derive");
     }
     p->feats_in = b.f32((size_t)B * T * e->feat_dim);
     p->emb = b.f32((size_t)B * e->embed_dim);
@@ -732,7 +727,7 @@ int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* pat
     for (size_t i = 0; i < p->ops.size(); ++i) {
         std::string lab = p->ops[i].label;
         for (char& ch : lab) if (ch == '"' || ch == '\\') ch = ' ';
-        j += std::string(i ? "," : "") + "{\"label\":\"" + lab + "\",\"trace\":" + (p->ops[i].trace.empty() ? std::string("null") : p->ops[i].trace) + "}";
+        j += std::string(i ? "," : "") + "{\"label\":\"" + lab + "\",\"trace\":" + (p->ops[i].trace ? p->ops[i].trace() : std::string("null")) + "}";
     }
     j += "]}";
     FILE* f = fopen(path, "wb");

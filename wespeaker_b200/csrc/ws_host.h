@@ -1,7 +1,10 @@
 // Host-side plumbing shared by the engine translation units: error reporting, activation views, the conv
 // operator builder (wgmma/TMA or FFMA), device allocation tracking.
 #pragma once
+#include <array>
 #include <cstdio>
+#include <cstdlib>
+#include <cstring>
 #include <functional>
 #include <map>
 #include <string>
@@ -41,37 +44,7 @@ struct PlanCheckScope {
     ~PlanCheckScope();
 };
 void* plan_check_alloc(size_t bytes);   // 256-byte aligned placeholder address
-// Plan-trace mode: the builders keep each op's JSON trace (PlanOp::trace).  On in plan-check mode and, on a real engine, with
-// the engine option plan_trace = 1 (ws_engine_plan_trace then writes real device addresses).  Thread-local like the above.
-bool plan_trace_mode();
-struct PlanTraceScope {
-    bool prev;
-    explicit PlanTraceScope(bool on);
-    ~PlanTraceScope();
-};
-
-// channels-last activation view: element (b,f,t,c) at p[((b*F+f)*T+t)*ld + c]
-struct View {
-    void* p = nullptr;
-    void* plo = nullptr;  // 3xTF32 mode: twin buffer holding x - tf32_trunc(x)
-    int B = 0, F = 1, T = 0, C = 0;
-    long long ld = 0;
-    int dt = WS_F32;
-    long long npos() const { return (long long)B * F * T; }
-    // the same buffer as a dense (B, F, T, C) tensor
-    View shaped(int b, int f, int t, int c) const {
-        View v = *this;
-        v.B = b; v.F = f; v.T = t; v.C = c; v.ld = c;
-        return v;
-    }
-    View ch(int c0, int c) const {
-        View v = *this;
-        v.p = (char*)p + (size_t)c0 * ws_esize(dt);
-        if (plo) v.plo = (char*)plo + (size_t)c0 * ws_esize(dt);
-        v.C = c;
-        return v;
-    }
-};
+using View = WsView;   // ws_kernels.cuh
 
 // one fused conv/GEMM launch
 struct ConvSpec {
@@ -97,14 +70,14 @@ int add_conv_taps(ConvSpec& spec, const View& x, int kf, int kt, int dil_f, int 
 
 using Op = std::function<const char*(cudaStream_t)>;
 // One op of a launch plan: the launch closure, a label and FLOPs (tuning aid, ws_engine_profile_ops; FLOPs 0 = not GEMM-like)
-// and, in plan-trace mode only, a JSON description of the op (operands as addresses, shapes, strides, epilogue) that
-// ws_engine_plan_trace writes so that a test can re-evaluate the plan's arithmetic on the host against the oracle, or check
-// what each kernel of a real engine wrote.
+// and a JSON description of the op (operands as addresses, shapes, strides, epilogue), made when ws_engine_plan_trace asks
+// for it, so that a test can re-evaluate the plan's arithmetic on the host against the oracle, or check what each kernel of
+// a real engine wrote.
 struct PlanOp {
     Op run;
     std::string label;
     double flops = 0;
-    std::string trace;
+    std::function<std::string()> trace;
 };
 
 // Plan-trace JSON fields: "name":address, "name":integer, "name":float (%.9g), "name":{view}.  Optional buffers - a 3xTF32
@@ -112,9 +85,73 @@ struct PlanOp {
 inline std::string tp(const char* n, const void* q) { char b[96]; snprintf(b, sizeof b, "\"%s\":%llu", n, (unsigned long long)q); return b; }
 inline std::string ti(const char* n, long long v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%lld", n, v); return b; }
 inline std::string tf(const char* n, double v) { char b[96]; snprintf(b, sizeof b, "\"%s\":%.9g", n, v); return b; }
+// a float operand of a kernel, in the fewest digits that read back as the same float (1e-4f -> 0.0001)
+inline std::string tff(const char* n, float v) {
+    char b[96];
+    for (int d = 1; d <= 9; ++d)
+        if (snprintf(b, sizeof b, "\"%s\":%.*g", n, d, (double)v) > 0 && strtof(strchr(b, ':') + 1, nullptr) == v) break;
+    return b;
+}
 inline std::string tplo(const char* n, const void* q) { return q ? "," + tp(n, q) : std::string(); }
 inline std::string tview(const char* n, const View& v) {
     return std::string("\"") + n + "\":{" + tp("p", v.p) + tplo("plo", v.plo) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
+}
+inline std::string tes(int dt) { return ti("es", ws_esize(dt)); }
+
+// The plan trace of each bandwidth op, from the record its launcher takes (ws_kernels.cuh)
+inline std::string trace_of(const WsConvert& a) { return "{\"kind\":\"convert\"," + tes(a.dt) + "," + tp("in", a.in) + "," + tp("out", a.out) + "," + ti("n", a.n) + tplo("out_lo", a.lo) + "}"; }
+inline std::string trace_of(const WsTstats& a) {
+    static const char* kern[] = {"scalar", "tmean8", "tstats8"};
+    return "{\"kind\":\"tstats\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("pre_scale", a.pre_scale) + "," + tp("pre_shift", a.pre_shift) + "," + tp("out", a.out) + "," +
+           ti("out_es", ws_esize(a.odt)) + "," + ti("out_ld", a.out_ld) + "," + ti("std_off", a.std_off) + "," + tff("eps", a.eps) + "," + tp("lens", a.lens) + ",\"kernel\":\"" + kern[a.kernel] +
+           "\"}";
+}
+inline std::string trace_of(const WsZeroTail& a) { return "{\"kind\":\"zero_tail\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("lens", a.lens) + "}"; }
+inline std::string trace_of(const WsLensDerive& a) { return "{\"kind\":\"lens_derive\"," + tp("lens", a.lens) + "," + ti("B", a.B) + "," + ti("T", a.T) + "," + ti("levels", a.levels) + "}"; }
+inline std::string trace_of(const WsLinear& a) {
+    return "{\"kind\":\"linear\"," + tp("in", a.in) + "," + ti("in_ld", a.in_ld) + "," + tp("in2", a.in2) + "," + ti("in2_ld", a.in2_ld) + "," + ti("rows_per_b", a.rows_per_b) + "," + tp("W", a.W) +
+           "," + tp("bias", a.bias) + "," + tp("out", a.out) + "," + ti("out_ld", a.out_ld) + "," + ti("R", a.R) + "," + ti("I", a.I) + "," + ti("O", a.O) + "," + ti("act", a.act) + tplo("wsp", a.wsp) +
+           ",\"kernel\":\"" + (a.kernel == WS_LINEAR_ROWS64 ? "rows64" : "rows16") + "\"}";
+}
+inline std::string trace_of(const WsScaleResidual& a) {
+    return "{\"kind\":\"scale_residual\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("gate", a.gate) + "," + tview("res", a.res) + "," + tview("out", a.out) + "}";
+}
+inline std::string trace_of(const WsAffCombine& a) {
+    return "{\"kind\":\"aff_combine\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tview("y", a.y) + "," + tview("t", a.t) + "," + tview("out", a.out) + "}";
+}
+inline std::string trace_of(const WsAstpStats& a) {
+    return "{\"kind\":\"astp_stats\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tview("logits", a.logits) + "," + tp("stats", a.stats) + "," + tp("lens", a.lens) + "," + tff("eps", a.var_floor) +
+           ",\"kernel\":\"" + (a.kernel == WS_ASTP_STATS4 ? "stats4" : "scalar") + "\"}";
+}
+inline std::string trace_of(const WsSimamStats& a) {
+    return "{\"kind\":\"simam_stats\"," + tes(a.y.dt) + "," + tview("x", a.y) + "," + tp("stats", a.stats) + "," + tp("lens", a.lens) + tplo("partial", a.partial) + "}";
+}
+inline std::string trace_of(const WsSimamApply& a) {
+    View res = a.y;   // res has y's extents, at res's own row pitch
+    res.p = const_cast<void*>(a.res); res.plo = nullptr; res.ld = a.rs.t;
+    return "{\"kind\":\"simam_apply\"," + tes(a.y.dt) + "," + tview("y", a.y) + "," + tp("stats", a.stats) + "," + tview("res", res) + "," + tp("out", a.out) + "," + ti("out_sb", a.os.b) + "," +
+           ti("out_sf", a.os.f) + "," + ti("out_st", a.os.t) + "," + tp("lens", a.lens) + "," + tff("lambda", a.lambda) + "}";
+}
+inline std::string trace_of(const WsDwconv3x3& a) {
+    return "{\"kind\":\"dwconv3x3\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tview("out", a.out) + "," + tp("w", a.w) + "," + tp("shift", a.shift) + "," + tp("lens", a.lens) + "}";
+}
+inline std::string trace_of(const WsBnRelu& a) {
+    return "{\"kind\":\"bnrelu\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("scale", a.scale) + "," + tp("shift", a.shift) + "," + tview("out", a.out) + "," + ti("C", a.x.C) + "}";
+}
+inline std::string trace_of(const WsStem& a) {
+    return "{\"kind\":\"stem\"," + tes(a.out.dt) + "," + tp("feats", a.feats) + "," + tp("w9", a.w9) + "," + tp("shift", a.shift) + "," + tview("out", a.out) + "," + ti("Fdim", a.out.F) + "," +
+           tp("lens", a.lens) + "}";
+}
+inline std::string trace_of(const WsSegMeans& a) {
+    return "{\"kind\":\"seg_means\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + ti("seg_len", a.seg_len) + "," + tp("mean", a.mean) + "," + tp("segmean", a.segmean) + "}";
+}
+inline std::string trace_of(const WsSeGate& a) {
+    return "{\"kind\":\"se_gate\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("W1", a.W1) + "," + tp("b1", a.b1) + "," + tp("W2t", a.W2t) + "," + tp("b2", a.b2) + "," + ti("H", a.H) + "," +
+           tp("gate", a.gate) + "," + tp("lens", a.lens) + "," + tp("colsum", a.colsum) + "}";
+}
+inline std::string trace_of(const WsCamGate& a) {
+    return "{\"kind\":\"cam_gate\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + ti("seg_len", a.seg_len) + "," + tp("W1", a.W1) + "," + tp("b1", a.b1) + "," + tp("W2", a.W2) + "," + tp("b2", a.b2) +
+           "," + ti("H", a.H) + "," + ti("G", a.G) + "," + tp("gate", a.gate) + "}";
 }
 
 // Build a launch closure for `spec`; use_tc selects a tensor-core kernel (needs dt-aligned shapes) else FFMA.
@@ -150,10 +187,13 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
 // Fused CAM++ dense layers (ws_cam_dense.cu).  cam_layer_fill builds one host-side layer descriptor (weights are device
 // pointers in the activation dtype: W1 [128][cin] with BN2 folded, Wl [32][3*128] tap-major; everything else fp32 device
 // arrays).  make_cam_dense_op launches layers [l0, l1) of a device-resident descriptor array over the concat buffer X
-// (B,1,T,Cmax).  Outside the kernel's envelope: T > 512, fp32 activations.
+// (B,1,T,Cmax); layers / weights: the same descriptors on the host and the (W1, Wl) each one's tensor maps were encoded
+// from, for the plan trace.  Outside the kernel's envelope: T > 512, fp32 activations.
+constexpr int kCamSegLen = 100;   // CAM++ context segments (campplus.py:108-135: seg_len)
 bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const float* bn1_scale, const float* bn1_shift,
                     const float* bias2, const float* w1c_t, const float* b1c, const float* w2c_t, const float* b2c, int cin,
                     int dil);
-OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, int l0, int l1, PlanOp* op, const int* lens = nullptr);
+OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std::vector<WsCamLayer>& layers,
+                          const std::vector<std::array<const void*, 2>>& weights, int l0, int l1, PlanOp* op, const int* lens = nullptr);
 
 }  // namespace ws

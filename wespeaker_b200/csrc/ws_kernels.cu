@@ -895,100 +895,120 @@ inline int grid_for(long long n, int block, int cap = 0) {
 
 }  // namespace
 
-const char* ws_launch_convert(const float* in, void* out, float* lo, int dt, long long n, cudaStream_t s) {
-    convert_kernel<<<grid_for(n, 256), 256, 0, s>>>(in, out, lo, dt, n);
+const char* ws_launch_convert(const WsConvert& a, cudaStream_t s) {
+    convert_kernel<<<grid_for(a.n, 256), 256, 0, s>>>(a.in, a.out, a.lo, a.dt, a.n);
     return last_err();
 }
 
-const char* ws_launch_tstats(const void* x, int dt, int B, int F, int T, int C, long long ld, const float* pre_scale,
-                             const float* pre_shift, void* out, int odt, long long out_ld, int std_off, float eps,
-                             cudaStream_t s, const int* lens) {
-    if (std_off < 0 && F == 1 && pre_scale == nullptr && odt == WS_F32 && C % 8 == 0 && lens == nullptr) {
-        dim3 g8((C + 511) / 512, B), b8(64, 8);
-        tmean8_kernel<<<g8, b8, 0, s>>>(x, dt, T, C, ld, (float*)out, out_ld);
+int ws_tstats_kernel(const WsTstats& a) {
+    const WsView& x = a.x;
+    if (a.std_off < 0 && x.F == 1 && a.pre_scale == nullptr && a.odt == WS_F32 && x.C % 8 == 0 && a.lens == nullptr) return WS_TSTATS_TMEAN8;
+    if (x.dt != WS_F32 && x.C % 8 == 0 && x.ld % 8 == 0 && ((uintptr_t)x.p & 15) == 0) return WS_TSTATS_8;
+    return WS_TSTATS_SCALAR;
+}
+
+const char* ws_launch_tstats(const WsTstats& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    if (a.kernel == WS_TSTATS_TMEAN8) {
+        dim3 g8((x.C + 511) / 512, x.B), b8(64, 8);
+        tmean8_kernel<<<g8, b8, 0, s>>>(x.p, x.dt, x.T, x.C, x.ld, (float*)a.out, a.out_ld);
         return last_err();
     }
-    if (dt != WS_F32 && C % 8 == 0 && ld % 8 == 0 && ((uintptr_t)x & 15) == 0) {
-        dim3 g8((C + 127) / 128, F, B), b8(16, 16);
-        if (dt == WS_BF16) tstats8_kernel<WS_BF16><<<g8, b8, 0, s>>>(x, F, T, C, ld, pre_scale, pre_shift, out, odt, out_ld, std_off, eps, lens);
-        else tstats8_kernel<WS_F16><<<g8, b8, 0, s>>>(x, F, T, C, ld, pre_scale, pre_shift, out, odt, out_ld, std_off, eps, lens);
+    if (a.kernel == WS_TSTATS_8) {
+        dim3 g8((x.C + 127) / 128, x.F, x.B), b8(16, 16);
+        if (x.dt == WS_BF16) tstats8_kernel<WS_BF16><<<g8, b8, 0, s>>>(x.p, x.F, x.T, x.C, x.ld, a.pre_scale, a.pre_shift, a.out, a.odt, a.out_ld, a.std_off, a.eps, a.lens);
+        else tstats8_kernel<WS_F16><<<g8, b8, 0, s>>>(x.p, x.F, x.T, x.C, x.ld, a.pre_scale, a.pre_shift, a.out, a.odt, a.out_ld, a.std_off, a.eps, a.lens);
         return last_err();
     }
-    dim3 grid((C + 31) / 32, F, B), block(32, 8);
-    tstats_kernel<<<grid, block, 0, s>>>(x, dt, F, T, C, ld, pre_scale, pre_shift, out, odt, out_ld, std_off, eps, lens);
+    dim3 grid((x.C + 31) / 32, x.F, x.B), block(32, 8);
+    tstats_kernel<<<grid, block, 0, s>>>(x.p, x.dt, x.F, x.T, x.C, x.ld, a.pre_scale, a.pre_shift, a.out, a.odt, a.out_ld, a.std_off, a.eps, a.lens);
     return last_err();
 }
 
-// the 64x64-tile kernel serves FC layers with enough rows and outputs to fill its tile and 16-byte aligned rows
-bool ws_linear_rows_big(long long in_ld, const float* in2, long long in2_ld, int R, int I, int O) {
-    return R >= 48 && O >= 48 && I % 4 == 0 && in_ld % 4 == 0 && (in2 == nullptr || in2_ld % 4 == 0);
+static dim3 linear_rows_grid(const WsLinear& a) {
+    const bool big = a.kernel == WS_LINEAR_ROWS64;
+    return dim3(big ? (a.O + 63) / 64 : (a.O + 31) / 32, big ? (a.R + 63) / 64 : (a.R + 15) / 16, a.nsplit < 1 ? 1 : a.nsplit);
 }
 
-const char* ws_launch_linear_rows(const float* in, long long in_ld, const float* in2, long long in2_ld,
-                                  int rows_per_b, const float* W, const float* bias, float* out, long long out_ld,
-                                  int R, int I, int O, int act, float* workspace, int nsplit, cudaStream_t s) {
-    const bool big = ws_linear_rows_big(in_ld, in2, in2_ld, R, I, O);
-    dim3 grid(big ? (O + 63) / 64 : (O + 31) / 32, big ? (R + 63) / 64 : (R + 15) / 16, nsplit < 1 ? 1 : nsplit);
-    auto kern = big ? linear_rows64_kernel : linear_rows_kernel;
+void ws_linear_rows_plan(WsLinear& a, int sms) {
+    // the 64x64-tile kernel serves FC layers with enough rows and outputs to fill its tile and 16-byte aligned rows
+    const bool big = a.R >= 48 && a.O >= 48 && a.I % 4 == 0 && a.in_ld % 4 == 0 && (a.in2 == nullptr || a.in2_ld % 4 == 0);
+    a.kernel = big ? WS_LINEAR_ROWS64 : WS_LINEAR_ROWS16;
+    a.nsplit = 1;
+    const dim3 g = linear_rows_grid(a);
+    const int blocks = (int)(g.x * g.y);
+    if (big) while (blocks * a.nsplit < sms && a.I / (a.nsplit * 2) >= 96 && a.nsplit < 32) a.nsplit *= 2;
+    else while (blocks * a.nsplit < 2 * sms && a.I / (a.nsplit * 2) >= 128 && a.nsplit < 16) a.nsplit *= 2;
+}
+
+const char* ws_launch_linear_rows(const WsLinear& a, cudaStream_t s) {
+    const dim3 grid = linear_rows_grid(a);
+    auto kern = a.kernel == WS_LINEAR_ROWS64 ? linear_rows64_kernel : linear_rows_kernel;
+    const int rpb = a.rows_per_b < 1 ? 1 : a.rows_per_b;
     if (grid.z == 1) {
-        kern<<<grid, 256, 0, s>>>(in, in_ld, in2, in2_ld, rows_per_b < 1 ? 1 : rows_per_b, W, bias, out, out_ld, R, I, O, act);
+        kern<<<grid, 256, 0, s>>>(a.in, a.in_ld, a.in2, a.in2_ld, rpb, a.W, a.bias, a.out, a.out_ld, a.R, a.I, a.O, a.act);
         return last_err();
     }
-    if (workspace == nullptr) return "linear_rows: split-K needs a workspace";
-    kern<<<grid, 256, 0, s>>>(in, in_ld, in2, in2_ld, rows_per_b < 1 ? 1 : rows_per_b, W, nullptr, workspace, O, R, I, O,
-                              WS_ACT_NONE);
-    const long long n = (long long)R * O;
-    linear_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(workspace, nsplit, bias, out, out_ld, R, O, act);
+    if (a.wsp == nullptr) return "linear_rows: split-K needs a workspace";
+    kern<<<grid, 256, 0, s>>>(a.in, a.in_ld, a.in2, a.in2_ld, rpb, a.W, nullptr, a.wsp, a.O, a.R, a.I, a.O, WS_ACT_NONE);
+    const long long n = (long long)a.R * a.O;
+    linear_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(a.wsp, a.nsplit, a.bias, a.out, a.out_ld, a.R, a.O, a.act);
     return last_err();
 }
 
-const char* ws_launch_scale_residual(const void* x, long long x_ld, const float* gate, const void* res,
-                                     long long res_ld, void* out, float* lo, long long out_ld, int dt, int B, int T,
-                                     int C, cudaStream_t s) {
+const char* ws_launch_scale_residual(const WsScaleResidual& a, cudaStream_t s) {
+    const int B = a.x.B, T = a.x.T, C = a.x.C;
     if (C % 8 != 0) return "scale_residual: C must be a multiple of 8";
     const long long nvec = (long long)B * T * (C / 8);
     if (nvec >= (1LL << 31)) return "scale_residual: tensor too large for 32-bit vector indices";
     const int g = grid_for(nvec, 256);
-    if (dt == WS_BF16) scale_residual_kernel<WS_BF16><<<g, 256, 0, s>>>(x, x_ld, gate, res, res_ld, out, lo, out_ld, T, C, nvec);
-    else if (dt == WS_F16) scale_residual_kernel<WS_F16><<<g, 256, 0, s>>>(x, x_ld, gate, res, res_ld, out, lo, out_ld, T, C, nvec);
-    else scale_residual_kernel<WS_F32><<<g, 256, 0, s>>>(x, x_ld, gate, res, res_ld, out, lo, out_ld, T, C, nvec);
+    const WsView &x = a.x, &r = a.res, &o = a.out;
+    if (x.dt == WS_BF16) scale_residual_kernel<WS_BF16><<<g, 256, 0, s>>>(x.p, x.ld, a.gate, r.p, r.ld, o.p, (float*)o.plo, o.ld, T, C, nvec);
+    else if (x.dt == WS_F16) scale_residual_kernel<WS_F16><<<g, 256, 0, s>>>(x.p, x.ld, a.gate, r.p, r.ld, o.p, (float*)o.plo, o.ld, T, C, nvec);
+    else scale_residual_kernel<WS_F32><<<g, 256, 0, s>>>(x.p, x.ld, a.gate, r.p, r.ld, o.p, (float*)o.plo, o.ld, T, C, nvec);
     return last_err();
 }
 
-const char* ws_launch_aff_combine(const void* x, long long x_ld, const void* y, long long y_ld, const void* t, long long t_ld,
-                                  void* out, float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s) {
-    if (C % 8 != 0 || x_ld % 8 != 0 || y_ld % 8 != 0 || t_ld % 8 != 0 || out_ld % 8 != 0) return "aff_combine: C and the row pitches must be multiples of 8";
-    const long long nvec = npos * (C / 8);
+const char* ws_launch_aff_combine(const WsAffCombine& a, cudaStream_t s) {
+    const WsView &x = a.x, &y = a.y, &t = a.t, &o = a.out;
+    const int C = x.C;
+    if (C % 8 != 0 || x.ld % 8 != 0 || y.ld % 8 != 0 || t.ld % 8 != 0 || o.ld % 8 != 0) return "aff_combine: C and the row pitches must be multiples of 8";
+    const long long nvec = x.npos() * (C / 8);
     if (nvec >= (1LL << 31)) return "aff_combine: tensor too large for 32-bit vector indices";
     const int g = grid_for(nvec, 256);
-    if (dt == WS_BF16) aff_combine_kernel<WS_BF16><<<g, 256, 0, s>>>(x, x_ld, y, y_ld, t, t_ld, out, lo, out_ld, C, nvec);
-    else if (dt == WS_F16) aff_combine_kernel<WS_F16><<<g, 256, 0, s>>>(x, x_ld, y, y_ld, t, t_ld, out, lo, out_ld, C, nvec);
-    else aff_combine_kernel<WS_F32><<<g, 256, 0, s>>>(x, x_ld, y, y_ld, t, t_ld, out, lo, out_ld, C, nvec);
+    float* lo = (float*)o.plo;
+    if (x.dt == WS_BF16) aff_combine_kernel<WS_BF16><<<g, 256, 0, s>>>(x.p, x.ld, y.p, y.ld, t.p, t.ld, o.p, lo, o.ld, C, nvec);
+    else if (x.dt == WS_F16) aff_combine_kernel<WS_F16><<<g, 256, 0, s>>>(x.p, x.ld, y.p, y.ld, t.p, t.ld, o.p, lo, o.ld, C, nvec);
+    else aff_combine_kernel<WS_F32><<<g, 256, 0, s>>>(x.p, x.ld, y.p, y.ld, t.p, t.ld, o.p, lo, o.ld, C, nvec);
     return last_err();
 }
 
-const char* ws_launch_astp_stats(const void* x, const void* logits, int dt, int B, int T, int C, long long ld,
-                                 float* out, float var_floor, cudaStream_t s, const int* lens) {
-    if (C % 2 != 0) return "astp_stats: C must be even";
-    if (C % 4 == 0 && ld % 4 == 0 && dt != WS_F32 && T <= 256) {
-        dim3 grid((C + 63) / 64, B), block(16, 32);
-        if (dt == WS_BF16) astp_stats4_kernel<WS_BF16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);
-        else astp_stats4_kernel<WS_F16><<<grid, block, 0, s>>>(x, logits, T, C, ld, out, var_floor, lens);
+int ws_astp_stats_kernel(const WsAstpStats& a) {
+    return a.x.C % 4 == 0 && a.x.ld % 4 == 0 && a.x.dt != WS_F32 && a.x.T <= 256 ? WS_ASTP_STATS4 : WS_ASTP_STATS_SCALAR;
+}
+
+const char* ws_launch_astp_stats(const WsAstpStats& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    if (x.C % 2 != 0) return "astp_stats: C must be even";
+    if (a.kernel == WS_ASTP_STATS4) {
+        dim3 grid((x.C + 63) / 64, x.B), block(16, 32);
+        if (x.dt == WS_BF16) astp_stats4_kernel<WS_BF16><<<grid, block, 0, s>>>(x.p, a.logits.p, x.T, x.C, x.ld, a.stats, a.var_floor, a.lens);
+        else astp_stats4_kernel<WS_F16><<<grid, block, 0, s>>>(x.p, a.logits.p, x.T, x.C, x.ld, a.stats, a.var_floor, a.lens);
         return last_err();
     }
-    dim3 grid((C + 63) / 64, B), block(32, 8);
-    astp_stats_kernel<<<grid, block, 0, s>>>(x, logits, dt, T, C, ld, out, var_floor, lens);
+    dim3 grid((x.C + 63) / 64, x.B), block(32, 8);
+    astp_stats_kernel<<<grid, block, 0, s>>>(x.p, a.logits.p, x.dt, x.T, x.C, x.ld, a.stats, a.var_floor, a.lens);
     return last_err();
 }
 
-const char* ws_launch_zero_tail(void* x, float* lo, int dt, int B, int F, int T, int C, long long ld, const int* lens,
-                                cudaStream_t s) {
-    if ((C * (dt == WS_F32 ? 4 : 2)) % 16 != 0 || (ld * (dt == WS_F32 ? 4 : 2)) % 16 != 0) return "zero_tail: rows must be 16-byte multiples";
-    zero_tail_kernel<<<dim3((unsigned)F, (unsigned)B), 256, 0, s>>>(x, lo, dt, F, T, C, ld, lens);
+const char* ws_launch_zero_tail(const WsZeroTail& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    if ((x.C * (x.dt == WS_F32 ? 4 : 2)) % 16 != 0 || (x.ld * (x.dt == WS_F32 ? 4 : 2)) % 16 != 0) return "zero_tail: rows must be 16-byte multiples";
+    zero_tail_kernel<<<dim3((unsigned)x.F, (unsigned)x.B), 256, 0, s>>>(x.p, (float*)x.plo, x.dt, x.F, x.T, x.C, x.ld, a.lens);
     return last_err();
 }
-const char* ws_launch_lens_derive(int* lens, int B, int T, int levels, cudaStream_t s) {
-    lens_derive_kernel<<<(B + 127) / 128, 128, 0, s>>>(lens, B, T, levels);
+const char* ws_launch_lens_derive(const WsLensDerive& a, cudaStream_t s) {
+    lens_derive_kernel<<<(a.B + 127) / 128, 128, 0, s>>>(a.lens, a.B, a.T, a.levels);
     return last_err();
 }
 const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, int frame_len, int shift, cudaStream_t s) {
@@ -996,44 +1016,45 @@ const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, in
     return last_err();
 }
 
-const char* ws_launch_bnrelu(const void* x, long long x_ld, const float* scale, const float* shift, void* out,
-                             float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s) {
-    const long long nvec = npos * (C / 4);
-    bnrelu_kernel<<<grid_for(nvec, 256), 256, 0, s>>>(x, x_ld, scale, shift, out, lo, out_ld, dt, C, nvec);
+const char* ws_launch_bnrelu(const WsBnRelu& a, cudaStream_t s) {
+    const WsView &x = a.x, &o = a.out;
+    const long long nvec = x.npos() * (x.C / 4);
+    bnrelu_kernel<<<grid_for(nvec, 256), 256, 0, s>>>(x.p, x.ld, a.scale, a.shift, o.p, (float*)o.plo, o.ld, x.dt, x.C, nvec);
     return last_err();
 }
 
-const char* ws_launch_stem(const float* feats, const float* w9, const float* shift, void* out, float* lo, int dt, int B,
-                           int T, int Fdim, int Cout, cudaStream_t s, const int* lens) {
+const char* ws_launch_stem(const WsStem& a, cudaStream_t s) {
+    const WsView& o = a.out;
+    const int B = o.B, T = o.T, Fdim = o.F;
     const dim3 grid((unsigned)((T + 127) / 128), (unsigned)((Fdim + 7) / 8), (unsigned)B);
     if (B > 65535) return "stem conv: batch too large for one launch";
-    if (Cout == 32) stem_kernel<32><<<grid, 128, 0, s>>>(feats, w9, shift, out, lo, dt, B, T, Fdim, lens);
-    else if (Cout == 64) stem_kernel<64><<<grid, 128, 0, s>>>(feats, w9, shift, out, lo, dt, B, T, Fdim, lens);
+    if (o.C == 32) stem_kernel<32><<<grid, 128, 0, s>>>(a.feats, a.w9, a.shift, o.p, (float*)o.plo, o.dt, B, T, Fdim, a.lens);
+    else if (o.C == 64) stem_kernel<64><<<grid, 128, 0, s>>>(a.feats, a.w9, a.shift, o.p, (float*)o.plo, o.dt, B, T, Fdim, a.lens);
     else return "stem conv supports 32 or 64 output channels";
     return last_err();
 }
 
-const char* ws_launch_seg_means(const void* x, int dt, int B, int T, int C, long long ld, int seg_len, float* mean,
-                                float* segmean, cudaStream_t s) {
-    dim3 grid((C + 31) / 32, B), block(32, 8);
-    seg_means_kernel<<<grid, block, 0, s>>>(x, dt, T, C, ld, seg_len, mean, segmean);
+const char* ws_launch_seg_means(const WsSegMeans& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    dim3 grid((x.C + 31) / 32, x.B), block(32, 8);
+    seg_means_kernel<<<grid, block, 0, s>>>(x.p, x.dt, x.T, x.C, x.ld, a.seg_len, a.mean, a.segmean);
     return last_err();
 }
 
-const char* ws_launch_cam_gate(const void* x, int dt, int B, int T, int C, long long ld, int seg_len, const float* W1,
-                               const float* b1, const float* W2, const float* b2, int H, int G, float* gate,
-                               cudaStream_t s) {
-    if (C != 128 || H != 64 || G != 32) return "cam_gate: expected C=128, H=64, G=32 (CAM++ bn_channels / reduction / growth)";
-    const int nseg = (T + seg_len - 1) / seg_len;
+const char* ws_launch_cam_gate(const WsCamGate& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    const int C = x.C, H = a.H;
+    if (C != 128 || H != 64 || a.G != 32) return "cam_gate: expected C=128, H=64, G=32 (CAM++ bn_channels / reduction / growth)";
+    const int nseg = (x.T + a.seg_len - 1) / a.seg_len;
     const size_t smem = (size_t)(H * C + nseg * C + 16 * C + nseg * H + C) * sizeof(float);
     if (smem > 48 * 1024) return "cam_gate: utterance too long for the shared-memory context buffer";
-    cam_gate_kernel<128, 64, 32><<<B, 256, smem, s>>>(x, dt, T, ld, seg_len, W1, b1, W2, b2, gate);
+    cam_gate_kernel<128, 64, 32><<<x.B, 256, smem, s>>>(x.p, x.dt, x.T, x.ld, a.seg_len, a.W1, a.b1, a.W2, a.b2, a.gate);
     return last_err();
 }
 
-const char* ws_launch_se_gate(const void* x, int dt, int B, int T, int C, long long ld, const float* W1, const float* b1,
-                              const float* W2t, const float* b2, int H, float* gate, const float* colsum, cudaStream_t s,
-                              const int* lens) {
+const char* ws_launch_se_gate(const WsSeGate& a, cudaStream_t s) {
+    const WsView& x = a.x;
+    const int C = x.C, H = a.H;
     if (H != 128 || (C != 512 && C != 1024 && C != 2048 && C != 256)) return "se_gate: expected H=128 and C in {256,512,1024,2048}";
     const size_t smem = (size_t)(2 * C + 8192 + 2 * H) * sizeof(float);
     static unsigned long long attr = 0;   // per-device opt-in (ws_common.cuh)
@@ -1043,8 +1064,8 @@ const char* ws_launch_se_gate(const void* x, int dt, int B, int T, int C, long l
         ws_dev_mark_init(&attr, dev);
     }
     if (smem > 96 * 1024) return "se_gate: channel count too large for shared memory";
-    if (colsum != nullptr && T < 128) return "se_gate: fused column sums need >= 128 frames per utterance";
-    if (lens != nullptr && colsum != nullptr) return "se_gate: fused column sums are not available for length-masked batches";
-    se_gate_kernel<128><<<(B + 1) / 2, 512, smem, s>>>(x, dt, B, T, C, ld, W1, b1, W2t, b2, gate, colsum, lens);
+    if (a.colsum != nullptr && x.T < 128) return "se_gate: fused column sums need >= 128 frames per utterance";
+    if (a.lens != nullptr && a.colsum != nullptr) return "se_gate: fused column sums are not available for length-masked batches";
+    se_gate_kernel<128><<<(x.B + 1) / 2, 512, smem, s>>>(x.p, x.dt, x.B, x.T, C, x.ld, a.W1, a.b1, a.W2t, a.b2, a.gate, a.colsum, a.lens);
     return last_err();
 }

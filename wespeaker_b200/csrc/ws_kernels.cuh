@@ -3,73 +3,119 @@
 #pragma once
 #include "ws_common.cuh"
 
-// ---- elementwise / reductions over channels-last activations [rows][ld]
-// (`lo`: optional fp32 twin receiving v - tf32_trunc(v) for the 3xTF32 GEMM path; pass nullptr otherwise)
-const char* ws_launch_convert(const float* in, void* out, float* lo, int dt, long long n, cudaStream_t s);
-// mean (and optional unbiased std, sqrt(var + eps)) over T for every (b, f, c).  x: [B][F][T][ld], channels [0,C).
-// Optional per-channel pre-affine + relu (CAM++ out_nonlinear, campplus.py:378-379).  Output (fp32 or `odt`):
+// ---- plan ops: one argument record per op kind, read by its launcher and by its plan-trace writer (ws_host.h).  Shape-dependent
+// kernel choices (*_kernel / *_plan) are made once, at plan build.  (`lo` / `plo`: optional fp32 twin receiving v - tf32_trunc(v)
+// for the 3xTF32 GEMM path; nullptr otherwise)
+
+// channels-last activation view: element (b,f,t,c) at p[((b*F+f)*T+t)*ld + c]
+struct WsView {
+    void* p = nullptr;
+    void* plo = nullptr;  // 3xTF32 mode: twin buffer holding x - tf32_trunc(x)
+    int B = 0, F = 1, T = 0, C = 0;
+    long long ld = 0;
+    int dt = WS_F32;
+    long long npos() const { return (long long)B * F * T; }
+    // the same buffer as a dense (B, F, T, C) tensor
+    WsView shaped(int b, int f, int t, int c) const {
+        WsView v = *this;
+        v.B = b; v.F = f; v.T = t; v.C = c; v.ld = c;
+        return v;
+    }
+    WsView ch(int c0, int c) const {
+        WsView v = *this;
+        v.p = (char*)p + (size_t)c0 * ws_esize(dt);
+        if (plo) v.plo = (char*)plo + (size_t)c0 * ws_esize(dt);
+        v.C = c;
+        return v;
+    }
+};
+
+struct WsConvert { const float* in; void* out; float* lo; int dt; long long n; };
+const char* ws_launch_convert(const WsConvert& a, cudaStream_t s);
+
+// mean (and optional unbiased std, sqrt(var + eps)) over T for every (b, f, c) of x's channels.  Optional per-channel
+// pre-affine + relu (CAM++ out_nonlinear, campplus.py:378-379).  Output (dtype odt):
 //   mean -> out[b*out_ld + c*F + f],  std -> out[b*out_ld + std_off + c*F + f]   (std skipped if std_off < 0)
-const char* ws_launch_tstats(const void* x, int dt, int B, int F, int T, int C, long long ld, const float* pre_scale,
-                             const float* pre_shift, void* out, int odt, long long out_ld, int std_off, float eps,
-                             cudaStream_t s, const int* lens = nullptr);
+enum WsTstatsKernel { WS_TSTATS_SCALAR, WS_TSTATS_TMEAN8, WS_TSTATS_8 };
+struct WsTstats { WsView x; const float* pre_scale; const float* pre_shift; void* out; int odt; long long out_ld; int std_off;
+    float eps; const int* lens; int kernel = WS_TSTATS_SCALAR; };
+int ws_tstats_kernel(const WsTstats& a);
+const char* ws_launch_tstats(const WsTstats& a, cudaStream_t s);
+
 // length-masked batches (per-utterance frame counts `lens`, device int32): zero the rows t >= lens[b]; derive the frame
 // counts behind stride-2 layers (lens is [levels][B], level 0 = input); frames from sample counts
-const char* ws_launch_zero_tail(void* x, float* lo, int dt, int B, int F, int T, int C, long long ld, const int* lens,
-                                cudaStream_t s);
-const char* ws_launch_lens_derive(int* lens, int B, int T, int levels, cudaStream_t s);
+struct WsZeroTail { WsView x; const int* lens; };
+const char* ws_launch_zero_tail(const WsZeroTail& a, cudaStream_t s);
+struct WsLensDerive { int* lens; int B, T, levels; };
+const char* ws_launch_lens_derive(const WsLensDerive& a, cudaStream_t s);
 const char* ws_launch_frames_from_samples(const int* nsamp, int* lens, int B, int Tmax, int frame_len, int shift, cudaStream_t s);
-// out[r][o] = act( sum_i W[o][i] * (in[r][i] + in2[r / rows_per_b][i]) + bias[o] ),  fp32 in/out, W fp32 [O][I]
-bool ws_linear_rows_big(long long in_ld, const float* in2, long long in2_ld, int R, int I, int O);
-const char* ws_launch_linear_rows(const float* in, long long in_ld, const float* in2, long long in2_ld,
-                                  int rows_per_b, const float* W, const float* bias, float* out, long long out_ld,
-                                  int R, int I, int O, int act, float* workspace, int nsplit, cudaStream_t s);
+
+// out[r][o] = act( sum_i W[o][i] * (in[r][i] + in2[r / rows_per_b][i]) + bias[o] ),  fp32 in/out, W fp32 [O][I]; split K
+// over nsplit CTAs (then wsp: fp32 [nsplit][R][O] partial sums)
+enum WsLinearKernel { WS_LINEAR_ROWS16, WS_LINEAR_ROWS64 };
+struct WsLinear { const float* in; long long in_ld; const float* in2; long long in2_ld; int rows_per_b; const float* W;
+    const float* bias; float* out; long long out_ld; int R, I, O, act; float* wsp; int nsplit = 1;
+    int kernel = WS_LINEAR_ROWS16; };
+// a.kernel and a.nsplit for a's shape: K is split so that the launch fills the `sms` SMs (these layers are latency-bound)
+void ws_linear_rows_plan(WsLinear& a, int sms);
+const char* ws_launch_linear_rows(const WsLinear& a, cudaStream_t s);
+
 // SE apply + residual (ecapa_tdnn.py:124,157): out[pos][c] = x[pos][c]*gate[b][c] + res[pos][c]
-const char* ws_launch_scale_residual(const void* x, long long x_ld, const float* gate, const void* res,
-                                     long long res_ld, void* out, float* lo, long long out_ld, int dt, int B, int T,
-                                     int C, cudaStream_t s);
+struct WsScaleResidual { WsView x; const float* gate; WsView res, out; };
+const char* ws_launch_scale_residual(const WsScaleResidual& a, cudaStream_t s);
+
 // ERes2Net AFF combine (eres2net.py:97-100): out[pos][c] = x * (1 + t) + y * (2 - (1 + t)), t = the tanh'd attention map
-const char* ws_launch_aff_combine(const void* x, long long x_ld, const void* y, long long y_ld, const void* t, long long t_ld,
-                                  void* out, float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s);
+struct WsAffCombine { WsView x, y, t, out; };
+const char* ws_launch_aff_combine(const WsAffCombine& a, cudaStream_t s);
+
 // ASTP statistics (pooling_layers.py:138-144): softmax over T of logits, weighted mean / std = sqrt(max(var, var_floor)) of x
-// (ECAPA's ASTP floors the variance at 1e-7, SimAM-ResNet's ASP at 1e-5, pooling_layers.py:198-203)
-const char* ws_launch_astp_stats(const void* x, const void* logits, int dt, int B, int T, int C, long long ld,
-                                 float* out /*[B][2C]*/, float var_floor, cudaStream_t s, const int* lens = nullptr);
+// (ECAPA's ASTP floors the variance at 1e-7, SimAM-ResNet's ASP at 1e-5, pooling_layers.py:198-203); logits are read with
+// x's row pitch
+enum WsAstpStatsKernel { WS_ASTP_STATS_SCALAR, WS_ASTP_STATS4 };
+struct WsAstpStats { WsView x, logits; float* stats /*[B][2C]*/; float var_floor; const int* lens;
+    int kernel = WS_ASTP_STATS_SCALAR; };
+int ws_astp_stats_kernel(const WsAstpStats& a);
+const char* ws_launch_astp_stats(const WsAstpStats& a, cudaStream_t s);
+
 // SimAM (ws_simam.cu, samresnet.py:65-70).  Statistics of y [B][F][T][ld] (channels [0,C)) per (b, c) over F x (its own
 // frames): stats fp32 [B][2][C] = mean, variance over n = F*T_b - 1; partial: fp32 scratch [B][F][C][2] (two launches).
-const char* ws_launch_simam_stats(const void* y, int dt, int B, int F, int T, int C, long long ld, float* partial, float* stats,
-                                  cudaStream_t s, const int* lens = nullptr);
+struct WsSimamStats { WsView y; float* partial; float* stats; const int* lens; };
+const char* ws_launch_simam_stats(const WsSimamStats& a, cudaStream_t s);
 // element (b, f, t, c) of a map at b*sb.b + f*sb.f + t*sb.t + c (elements)
-struct WsMapStrides {
-    long long b, f, t;
-};
-// out = relu(y * sigmoid((y - mean)^2 / (4 (var + lambda_p)) + 0.5) + res); res may alias out; rows t >= lens[b] of out are
-// zeroed; out_lo (optional, fp32 with out's strides) receives the 3xTF32 low part
-const char* ws_launch_simam_apply(const void* y, long long y_ld, const float* stats, float lambda_p, const void* res, WsMapStrides rs,
-                                  void* out, float* out_lo, WsMapStrides os, int dt, int B, int F, int T, int C, cudaStream_t s,
-                                  const int* lens = nullptr);
-// Depthwise 3x3 pad-1 conv + folded BN + ReLU (ws_dwconv.cu, gemini_dfresnet.py:37-44): out = relu(dwconv(x, w) + shift) with
-// w fp32 [C][3][3], shift fp32 [C]; rows t >= lens[b] are read as zeros and written as zeros; out_lo (fp32 activations,
-// optional) receives the 3xTF32 low part.  C % 8 == 0 in 16-bit, C % 4 == 0 in fp32.
-const char* ws_launch_dwconv3x3(const void* x, long long x_ld, const float* w, const float* shift, void* out, float* out_lo,
-                                long long out_ld, int dt, int B, int F, int T, int C, cudaStream_t s, const int* lens = nullptr);
-// out[pos][c] = relu(x[pos][c]*scale[c] + shift[c])  (CAM++ pre-activation BN-ReLU, campplus.py:164-166,214)
-const char* ws_launch_bnrelu(const void* x, long long x_ld, const float* scale, const float* shift, void* out,
-                             float* lo, long long out_ld, int dt, long long npos, int C, cudaStream_t s);
-// ResNet / FCM stem: Conv2d(1->Cout,3x3,pad 1) + folded BN + ReLU.  feats fp32 [B][T][Fdim] -> out [B][Fdim][T][Cout]
-const char* ws_launch_stem(const float* feats, const float* w9 /*[Cout][9]*/, const float* shift, void* out, float* lo,
-                           int dt, int B, int T, int Fdim, int Cout, cudaStream_t s, const int* lens = nullptr);
-// CAM context (campplus.py:108-135): mean over T and per-segment (seg_len) means with ceil-mode partial segment
-const char* ws_launch_seg_means(const void* x, int dt, int B, int T, int C, long long ld, int seg_len, float* mean,
-                                float* segmean /*[B][nseg][C]*/, cudaStream_t s);
+struct WsMapStrides { long long b, f, t; };
+// out = relu(y * sigmoid((y - mean)^2 / (4 (var + lambda)) + 0.5) + res) with y's extents; res may alias out; rows
+// t >= lens[b] of out are zeroed; out_lo (optional, fp32 with out's strides) receives the 3xTF32 low part
+struct WsSimamApply { WsView y; const float* stats; float lambda; const void* res; WsMapStrides rs; void* out; float* out_lo;
+    WsMapStrides os; const int* lens; };
+const char* ws_launch_simam_apply(const WsSimamApply& a, cudaStream_t s);
 
-// fused SE gate: gate[b][c] = sigmoid(W2 relu(W1 mean_T(x[b]) + b1) + b2); W2t is W2 transposed to [H][C]
-const char* ws_launch_se_gate(const void* x, int dt, int B, int T, int C, long long ld, const float* W1, const float* b1,
-                              const float* W2t, const float* b2, int H, float* gate, const float* colsum, cudaStream_t s,
-                              const int* lens = nullptr);
+// Depthwise 3x3 pad-1 conv + folded BN + ReLU (ws_dwconv.cu, gemini_dfresnet.py:37-44): out = relu(dwconv(x, w) + shift) with
+// w fp32 [C][3][3], shift fp32 [C], x's extents and dtype; rows t >= lens[b] are read as zeros and written as zeros; out.plo
+// (fp32 activations, optional) receives the 3xTF32 low part.  C % 8 == 0 in 16-bit, C % 4 == 0 in fp32.
+struct WsDwconv3x3 { WsView x; const float* w; const float* shift; WsView out; const int* lens; };
+const char* ws_launch_dwconv3x3(const WsDwconv3x3& a, cudaStream_t s);
+
+// out[pos][c] = relu(x[pos][c]*scale[c] + shift[c]) over x's channels (CAM++ pre-activation BN-ReLU, campplus.py:164-166,214)
+struct WsBnRelu { WsView x; const float* scale; const float* shift; WsView out; };
+const char* ws_launch_bnrelu(const WsBnRelu& a, cudaStream_t s);
+
+// ResNet / FCM stem: Conv2d(1->Cout,3x3,pad 1) + folded BN + ReLU.  feats fp32 [B][T][Fdim] -> out (B, Fdim, T, Cout)
+struct WsStem { const float* feats; const float* w9 /*[Cout][9]*/; const float* shift; WsView out; const int* lens; };
+const char* ws_launch_stem(const WsStem& a, cudaStream_t s);
+
+// CAM context (campplus.py:108-135): mean over T and per-segment (seg_len) means with ceil-mode partial segment
+struct WsSegMeans { WsView x; int seg_len; float* mean; float* segmean /*[B][nseg][C]*/; };
+const char* ws_launch_seg_means(const WsSegMeans& a, cudaStream_t s);
+
+// fused SE gate: gate[b][c] = sigmoid(W2 relu(W1 mean_T(x[b]) + b1) + b2); W2t is W2 transposed to [H][C]; colsum: the
+// per-unit column sums of x that the producing conv's epilogue wrote (instead of a pass over x), or nullptr
+struct WsSeGate { WsView x; const float* W1; const float* b1; const float* W2t; const float* b2; int H; float* gate;
+    const float* colsum; const int* lens; };
+const char* ws_launch_se_gate(const WsSeGate& a, cudaStream_t s);
 // fused CAM context gate: gate[b][seg][g] = sigmoid(W2 relu(W1 (mean_T(x) + segmean(x)) + b1) + b2)
-const char* ws_launch_cam_gate(const void* x, int dt, int B, int T, int C, long long ld, int seg_len, const float* W1,
-                               const float* b1, const float* W2, const float* b2, int H, int G, float* gate,
-                               cudaStream_t s);
+struct WsCamGate { WsView x; int seg_len; const float* W1; const float* b1; const float* W2; const float* b2; int H, G;
+    float* gate; };
+const char* ws_launch_cam_gate(const WsCamGate& a, cudaStream_t s);
 
 // ---- fbank + CMN (ws_fbank.cu)
 // 25 ms frame length / 10 ms shift in samples at sample_rate 8000 or 16000 (0 for any other rate)

@@ -50,7 +50,7 @@ struct Plan {
     int lane = 0;               // which of the engine's streams runs this plan through the device-pointer entry points
     cudaEvent_t done = nullptr; // recorded after every use: a later use on another stream waits for it
     bool check = false;         // built by a plan-check engine: buffers are placeholder addresses, nothing to release
-    // plan-trace engines (option plan_trace): every buffer this plan allocated, (address, bytes), for ws_engine_plan_trace
+    // every device buffer this plan allocated, (address, bytes), for ws_engine_plan_trace on real engines
     std::vector<std::pair<unsigned long long, unsigned long long>> trace_allocs;
     ~Plan() {
         if (done) cudaEventDestroy(done);
@@ -276,7 +276,7 @@ struct Builder {
             if (ok) set_err("cudaMalloc failed for an activation buffer");
             ok = false;
             return nullptr;
-        } else if (plan_trace_mode()) {
+        } else {
             p.trace_allocs.push_back({(unsigned long long)d, (unsigned long long)bytes});
         }
         p.bufs.push_back(d);
@@ -302,19 +302,16 @@ struct Builder {
         return v;
     }
     void push(PlanOp op) { p.ops.push_back(std::move(op)); }
-    // a bandwidth op: launch closure, label, and its plan-trace description (kept in plan-trace mode only)
-    void push(Op run, const char* label, std::string trace) {
-        push(PlanOp{std::move(run), label, 0.0, plan_trace_mode() ? std::move(trace) : std::string()});
+    // a bandwidth op: its argument record, which both its launch and its plan trace (trace_of, ws_host.h) read
+    template <class Rec>
+    void push(const Rec& a, const char* (*launch)(const Rec&, cudaStream_t), const char* label) {
+        push(PlanOp{[a, launch](cudaStream_t s) { return launch(a, s); }, label, 0.0, [a] { return trace_of(a); }});
     }
     // length-masked plans: frame counts of stride level k (nullptr in ordinary plans), and "zero the rows behind every
     // utterance's end" for tensors a time-mixing op is about to read (the reference's unpadded forward sees zero padding)
     const int* lens(int level) const { return p.masked ? p.lens + (size_t)level * p.B : nullptr; }
     void zero_tail(const View& v, int level) {
-        if (!p.masked) return;
-        const View x = v;
-        const int* l = lens(level);
-        push([=](cudaStream_t s) { return ws_launch_zero_tail(x.p, (float*)x.plo, x.dt, x.B, x.F, x.T, x.C, x.ld, l, s); }, "zero_tail",
-             "{\"kind\":\"zero_tail\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("lens", l) + "}");
+        if (p.masked) push(WsZeroTail{v, lens(level)}, ws_launch_zero_tail, "zero_tail");
     }
     void conv(const ConvSpec& s_in) {
         if (!good()) return;
@@ -352,50 +349,23 @@ struct Builder {
     }
     void tstats(const View& x, const float* pre_scale, const float* pre_shift, float* out, long long out_ld, int std_off,
                 int level = 0) {
-        View xv = x;
-        const int* l = lens(level);
-        push([=](cudaStream_t s) {
-            return ws_launch_tstats(xv.p, xv.dt, xv.B, xv.F, xv.T, xv.C, xv.ld, pre_scale, pre_shift, out, WS_F32, out_ld,
-                                    std_off, 1e-7f, s, l);
-        }, "tstats", "{\"kind\":\"tstats\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("pre_scale", pre_scale) + "," + tp("pre_shift", pre_shift) + "," +
-                     tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("std_off", std_off) + "," + tp("lens", l) + "}");
+        WsTstats a{x, pre_scale, pre_shift, out, WS_F32, out_ld, std_off, 1e-7f, lens(level)};
+        a.kernel = ws_tstats_kernel(a);
+        push(a, ws_launch_tstats, "tstats");
     }
     void linear(const float* in, long long in_ld, const float* in2, long long in2_ld, int rows_per_b, const float* W,
                 const float* bias, float* out, long long out_ld, int R, int I, int O, int act) {
-        // split K so that the launch fills the machine (these layers are latency-bound otherwise)
-        const bool big = ws_linear_rows_big(in_ld, in2, in2_ld, R, I, O);
-        const int blocks = big ? ((O + 63) / 64) * ((R + 63) / 64) : ((O + 31) / 32) * ((R + 15) / 16);
-        int nsplit = 1;
-        const int sms = ws_num_sms();
-        if (big) while (blocks * nsplit < sms && I / (nsplit * 2) >= 96 && nsplit < 32) nsplit *= 2;
-        else while (blocks * nsplit < 2 * sms && I / (nsplit * 2) >= 128 && nsplit < 16) nsplit *= 2;
-        float* wsp = nsplit > 1 ? f32((size_t)nsplit * R * O) : nullptr;
-        if (nsplit > 1) p.extra_launches += 1;
-        push([=](cudaStream_t s) {
-            return ws_launch_linear_rows(in, in_ld, in2, in2_ld, rows_per_b, W, bias, out, out_ld, R, I, O, act, wsp,
-                                         nsplit, s);
-        }, "linear_rows", "{\"kind\":\"linear\"," + tp("in", in) + "," + ti("in_ld", in_ld) + "," + tp("in2", in2) + "," + ti("in2_ld", in2_ld) + "," + ti("rows_per_b", rows_per_b) + "," +
-                     tp("W", W) + "," + tp("bias", bias) + "," + tp("out", out) + "," + ti("out_ld", out_ld) + "," + ti("R", R) + "," + ti("I", I) + "," + ti("O", O) + "," + ti("act", act) +
-                     tplo("wsp", wsp) + "}");
+        WsLinear a{in, in_ld, in2, in2_ld, rows_per_b, W, bias, out, out_ld, R, I, O, act, nullptr};
+        ws_linear_rows_plan(a, ws_num_sms());
+        if (a.nsplit > 1) {
+            a.wsp = f32((size_t)a.nsplit * R * O);
+            p.extra_launches += 1;
+        }
+        push(a, ws_launch_linear_rows, "linear_rows");
     }
     // the fp32 input features -> x0 (B,1,T,feat_dim) in the activation dtype
     void convert_input(const View& x0) {
-        const float* fin = p.feats_in;
-        void* xo = x0.p;
-        float* xlo = (float*)x0.plo;
-        const int dt = x0.dt;
-        const long long n = x0.npos() * x0.C;
-        push([=](cudaStream_t s) { return ws_launch_convert(fin, xo, xlo, dt, n, s); }, "convert",
-             "{\"kind\":\"convert\"," + ti("es", ws_esize(dt)) + "," + tp("in", fin) + "," + tp("out", xo) + "," + ti("n", n) + tplo("out_lo", xlo) + "}");
-    }
-    // out = relu(x * scale + shift), per channel over x's C channels
-    void bnrelu(const View& x, const float* scale, const float* shift, const View& out) {
-        const View xv = x, ov = out;
-        const int C = x.C;
-        const long long npos = x.npos();
-        push([=](cudaStream_t s) { return ws_launch_bnrelu(xv.p, xv.ld, scale, shift, ov.p, (float*)ov.plo, ov.ld, xv.dt, npos, C, s); }, "bnrelu",
-             "{\"kind\":\"bnrelu\"," + ti("es", ws_esize(x.dt)) + "," + tview("x", x) + "," + tp("scale", scale) + "," + tp("shift", shift) + "," +
-             tview("out", out) + "," + ti("C", C) + "}");
+        push(WsConvert{p.feats_in, x0.p, (float*)x0.plo, x0.dt, x0.npos() * x0.C}, ws_launch_convert, "convert");
     }
     // The halo-resident 3x3 pad-1 conv (ws_conv3x3.cu: every input row crosses L2 -> SM once instead of once per tap),
     // out = act(conv(x, W) + bias [+ res]).  halo3x3: whether the precision and the options let convs use it.  halo_conv3x3
@@ -461,11 +431,9 @@ struct Builder {
         ep.bias = bias2;
         conv_simple(h, logits, W2, 1, 1, 1, 1, 0, 0, 1, 1, ep);
         if (!good()) return false;
-        const View fr = x, lg = logits;
-        const float var_floor = (float)eps;
-        push([=](cudaStream_t s) { return ws_launch_astp_stats(fr.p, lg.p, fr.dt, fr.B, fr.T, fr.C, fr.ld, stats, var_floor, s, l); }, "astp_stats",
-             "{\"kind\":\"astp_stats\"," + ti("es", ws_esize(fr.dt)) + "," + tview("x", fr) + "," + tview("logits", lg) + "," + tp("stats", stats) + "," +
-             tp("lens", l) + "," + tf("eps", eps) + "}");
+        WsAstpStats a{x, logits, stats, (float)eps, l};
+        a.kernel = ws_astp_stats_kernel(a);
+        push(a, ws_launch_astp_stats, "astp_stats");
         return good();
     }
 };

@@ -164,39 +164,41 @@ bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 }  // namespace
 
-const char* ws_launch_simam_stats(const void* y, int dt, int B, int F, int T, int C, long long ld, float* partial, float* stats,
-                                  cudaStream_t s, const int* lens) {
-    if (C % 8 != 0 || ld % 8 != 0 || !aligned16(y) || !aligned16(partial)) return "simam_stats: C and ld must be multiples of 8, buffers 16-byte aligned";
+const char* ws_launch_simam_stats(const WsSimamStats& a, cudaStream_t s) {
+    const WsView& y = a.y;
+    const int B = y.B, F = y.F, T = y.T, C = y.C;
+    if (C % 8 != 0 || y.ld % 8 != 0 || !aligned16(y.p) || !aligned16(a.partial)) return "simam_stats: C and ld must be multiples of 8, buffers 16-byte aligned";
     if (F < 1 || T < 1 || F > 65535 || B > 65535 || (long long)F * T < 2) return "simam_stats: bad extents";
     const dim3 grid((C + kCBlk - 1) / kCBlk, F, B), block(8, kSlices);
-    if (dt == WS_BF16) simam_partial_kernel<WS_BF16><<<grid, block, 0, s>>>(y, F, T, C, ld, partial, lens);
-    else if (dt == WS_F16) simam_partial_kernel<WS_F16><<<grid, block, 0, s>>>(y, F, T, C, ld, partial, lens);
-    else simam_partial_kernel<WS_F32><<<grid, block, 0, s>>>(y, F, T, C, ld, partial, lens);
-    simam_merge_kernel<<<dim3((C + 127) / 128, B), 128, 0, s>>>(partial, F, T, C, stats, lens);
+    if (y.dt == WS_BF16) simam_partial_kernel<WS_BF16><<<grid, block, 0, s>>>(y.p, F, T, C, y.ld, a.partial, a.lens);
+    else if (y.dt == WS_F16) simam_partial_kernel<WS_F16><<<grid, block, 0, s>>>(y.p, F, T, C, y.ld, a.partial, a.lens);
+    else simam_partial_kernel<WS_F32><<<grid, block, 0, s>>>(y.p, F, T, C, y.ld, a.partial, a.lens);
+    simam_merge_kernel<<<dim3((C + 127) / 128, B), 128, 0, s>>>(a.partial, F, T, C, a.stats, a.lens);
     return last_err();
 }
 
-const char* ws_launch_simam_apply(const void* y, long long y_ld, const float* stats, float lambda_p, const void* res, WsMapStrides rs,
-                                  void* out, float* out_lo, WsMapStrides os, int dt, int B, int F, int T, int C, cudaStream_t s,
-                                  const int* lens) {
-    if (C % 8 != 0 || y_ld % 8 != 0 || rs.b % 8 || rs.f % 8 || rs.t % 8 || os.b % 8 || os.f % 8 || os.t % 8 ||
-        !aligned16(y) || !aligned16(res) || !aligned16(out) || !aligned16(stats) || (out_lo && !aligned16(out_lo)))
+const char* ws_launch_simam_apply(const WsSimamApply& a, cudaStream_t s) {
+    const WsView& y = a.y;
+    const WsMapStrides &rs = a.rs, &os = a.os;
+    const int F = y.F, T = y.T, C = y.C;
+    if (C % 8 != 0 || y.ld % 8 != 0 || rs.b % 8 || rs.f % 8 || rs.t % 8 || os.b % 8 || os.f % 8 || os.t % 8 ||
+        !aligned16(y.p) || !aligned16(a.res) || !aligned16(a.out) || !aligned16(a.stats) || (a.out_lo && !aligned16(a.out_lo)))
         return "simam_apply: C and every stride must be multiples of 8, buffers 16-byte aligned";
-    const long long nvec = (long long)B * F * T * (C / 8);
+    const long long nvec = y.npos() * (C / 8);
     if (nvec >= (1LL << 31)) return "simam_apply: tensor too large for 32-bit vector indices";
     const int g = (int)std::min<long long>((nvec + 255) / 256, (long long)ws_num_sms() * 16);
-    if (dt == WS_BF16) simam_apply_kernel<WS_BF16><<<g, 256, 0, s>>>(y, y_ld, stats, lambda_p, res, rs, out, out_lo, os, F, T, C, lens, nvec);
-    else if (dt == WS_F16) simam_apply_kernel<WS_F16><<<g, 256, 0, s>>>(y, y_ld, stats, lambda_p, res, rs, out, out_lo, os, F, T, C, lens, nvec);
-    else simam_apply_kernel<WS_F32><<<g, 256, 0, s>>>(y, y_ld, stats, lambda_p, res, rs, out, out_lo, os, F, T, C, lens, nvec);
+    if (y.dt == WS_BF16) simam_apply_kernel<WS_BF16><<<g, 256, 0, s>>>(y.p, y.ld, a.stats, a.lambda, a.res, rs, a.out, a.out_lo, os, F, T, C, a.lens, nvec);
+    else if (y.dt == WS_F16) simam_apply_kernel<WS_F16><<<g, 256, 0, s>>>(y.p, y.ld, a.stats, a.lambda, a.res, rs, a.out, a.out_lo, os, F, T, C, a.lens, nvec);
+    else simam_apply_kernel<WS_F32><<<g, 256, 0, s>>>(y.p, y.ld, a.stats, a.lambda, a.res, rs, a.out, a.out_lo, os, F, T, C, a.lens, nvec);
     return last_err();
 }
 
 extern "C" int ws_simam(const ws_simam_desc* d, void* stream) {
     if (!d || !d->y || !d->res || !d->out || !d->stats || !d->partial) { ws::set_err("ws_simam: null argument"); return 1; }
     cudaStream_t s = (cudaStream_t)stream;
-    WS_CKS(ws_launch_simam_stats(d->y, d->dtype, d->B, d->F, d->T, d->C, d->y_ld, d->partial, d->stats, s, d->lens));
-    const WsMapStrides rs{d->res_sb, d->res_sf, d->res_st}, os{d->out_sb, d->out_sf, d->out_st};
-    WS_CKS(ws_launch_simam_apply(d->y, d->y_ld, d->stats, d->lambda_p, d->res, rs, d->out, (float*)d->out_lo, os, d->dtype, d->B, d->F, d->T,
-                                 d->C, s, d->lens));
+    const WsView y{const_cast<void*>(d->y), nullptr, d->B, d->F, d->T, d->C, d->y_ld, d->dtype};
+    WS_CKS(ws_launch_simam_stats(WsSimamStats{y, d->partial, d->stats, d->lens}, s));
+    WS_CKS(ws_launch_simam_apply(WsSimamApply{y, d->stats, d->lambda_p, d->res, {d->res_sb, d->res_sf, d->res_st}, d->out, (float*)d->out_lo,
+                                              {d->out_sb, d->out_sf, d->out_st}, d->lens}, s));
     return 0;
 }
