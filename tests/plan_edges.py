@@ -5,44 +5,40 @@ of those branches, and tests/test_plan_edges.py checks on the CPU that every bra
 moving a threshold names the branch that lost its coverage."""
 
 
-def _label_fields(label):
-    return dict(w.split("=", 1) for w in label.split() if "=" in w)
-
-
 def op_branches(op):
-    """the kernel-geometry branch keys one traced op (label + trace) takes"""
-    tr, lab = op["trace"], op["label"]
-    kind = tr["kind"]
+    """the kernel-geometry branch keys one traced op takes: the geometry the host chose (the trace's "launch"), and the
+    extents where a kernel's own constants decide"""
+    tr = op["trace"]
+    kind, g = tr["kind"], tr.get("launch", {})
     out = set()
     masked = bool(tr.get("lens"))
-    if kind == "conv3x3":       # make_conv3x3_op (ws_conv_host.cu): geometry in the label
-        f = _label_fields(lab)
-        B, T, nb, nmt, st = int(f["B"]), int(f["T"]), int(f["nb"]), int(f["n_mt"]), tr["st"]
-        if f["caseB"] == "1":
+    if kind == "conv3x3":       # make_conv3x3_op (ws_conv_host.cu)
+        B, T = tr["out"]["B"], tr["out"]["T"]
+        if g["case_b"]:
             out.add("conv3x3:caseB")
-            if B % nb:
+            if B % g["nb"]:
                 out.add("conv3x3:caseB-ragged" + ("-masked" if masked else ""))
-        elif st == 2:
-            out.add("conv3x3:stride2-ttiles=%s" % ("1" if T <= 128 else ">1"))
-        elif T <= 256:
-            out.add(f"conv3x3:n_mt={nmt}")
-            if T + 2 > 256:
+        elif tr["st"] == 2:
+            out.add("conv3x3:stride2-ttiles=%s" % ("1" if g["n_tt"] == 1 else ">1"))
+        elif g["n_tt"] == 1:
+            out.add(f"conv3x3:n_mt={g['n_mt']}")
+            if g["tb"] + 2 > 256:
                 out.add("conv3x3:multibox")
         else:
-            tb = 256 if nmt == 2 else 128
-            out.add(f"conv3x3:ttile={tb}")
-            if T % tb == 1:
-                out.add(f"conv3x3:ttile={tb}-tail=1")
+            out.add(f"conv3x3:ttile={g['tb']}")
+            if T % g["tb"] == 1:
+                out.add(f"conv3x3:ttile={g['tb']}-tail=1")
         if T == 1:
             out.add("conv3x3:T=1")
     elif kind == "conv":        # make_conv_op / tc2_geometry (ws_conv_host.cu)
         pos = tr["B"] * tr["F"] * tr["T"]
-        kern = lab.split()[0]
-        if kern == "conv_tc3":
+        if g["kernel"] == "tc3":
             out.add("conv:cluster")
             if ((pos + 127) // 128) % 2:
                 out.add("conv:cluster-odd-tiles")
-        if kern == "conv_tc2" and 132 * 128 - 128 <= pos < 132 * 128:
+            if g["bn"] == 256:      # the 256-wide N tile on clusters
+                out.add("conv:bn=256")
+        if g["kernel"] == "tc2" and 132 * 128 - 128 <= pos < 132 * 128:
             out.add("conv:just-below-cluster")
         flat = len(tr["taps"]) == 1 and tr["taps"][0][2] == 0 and tr["taps"][0][3] == 0
         if flat and pos % 128 == 1:
@@ -53,12 +49,9 @@ def op_branches(op):
             out.add("conv:empty-plane")
         if tr.get("colsum"):
             out.add("conv:se-colsum")
-        if "bn=256" in lab.split():
-            out.add("conv:bn=256")
-    elif kind == "res2_fused":  # make_res2_op: ntile
-        T = tr["x"]["T"]
-        out.add("res2:ntile=%d" % (1 if T <= 256 else (T + 191) // 192))
-        if T < 7 * tr["dil"]:
+    elif kind == "res2_fused":  # make_res2_op: time tiles
+        out.add("res2:ntile=%d" % g["ntile"])
+        if tr["x"]["T"] < 7 * tr["dil"]:
             out.add("res2:T<7dil")
     elif kind == "astp_fused":  # 256-frame online-softmax chunks
         T = tr["x"]["T"]
@@ -67,30 +60,29 @@ def op_branches(op):
         if n > 1 and T % 256 == 1:
             out.add("astp_fused:tail=1")
     elif kind == "astp_stats":  # the kernel the plan chose (ws_astp_stats_kernel)
-        out.add("astp_stats:" + tr["kernel"])
+        out.add("astp_stats:" + g["kernel"])
     elif kind == "se_gate":     # two utterances per CTA
         if tr["x"]["B"] % 2:
             out.add("se_gate:odd-B")
         if tr["x"]["T"] < 128:
             out.add("se_gate:T<128")
     elif kind == "tstats":      # the kernel the plan chose (ws_tstats_kernel)
-        k = tr["kernel"]
+        k = g["kernel"]
         if k == "tstats8":
             T = tr["x"]["T"]    # tstats8's 4-wide loop runs while t + 48 < T, t = slice (0..15) + 64 k
             out.add("tstats8:" + ("T<=48" if T <= 48 else "49<=T<64" if T < 64 else "T>=64"))
         else:
             out.add("tmean8" if k == "tmean8" else "tstats:" + k)
     elif kind == "linear":      # the kernel the plan chose (ws_linear_rows_plan); split-K when the launch would not fill the SMs
-        out.add("linear:" + tr["kernel"])
+        out.add("linear:" + g["kernel"])
         if tr.get("wsp"):
             out.add("linear:split-K")
     elif kind == "stem":        # 128-frame tiles
         T = tr["out"]["T"]
         out.add("stem:T<128" if T < 128 else "stem:ragged-tiles" if T % 128 else "stem:whole-tiles")
-    elif kind == "cam_dense":   # make_cam_dense_op: ceil(T'/128) M tiles, T' <= 512
-        T = tr["X"]["T"]
-        out.add(f"cam_dense:nmt={(T + 127) // 128}")
-        if T % 100 == 1:
+    elif kind == "cam_dense":   # make_cam_dense_op: M tiles of 128 frames, T' <= 512
+        out.add(f"cam_dense:nmt={g['nmt']}")
+        if tr["X"]["T"] % 100 == 1:
             out.add("cam_dense:seg-tail=1")
     elif kind in ("cam_gate", "seg_means"):     # the dense layers unfused (T' > 512 in 16-bit plans)
         if tr["es"] == 2:
@@ -122,7 +114,7 @@ def case_branches(ops, n_frames):
 
 
 # branches that depend on the SM count or the number of co-resident clusters: the plan-check engine (no device) cannot
-# predict them, so only the GPU test asserts them, from the real engine's labels
+# predict them, so only the GPU test asserts them, from the real engine's traces
 DEVICE_ONLY = {"conv:bn=256", "linear:split-K"}
 
 # every branch some edge case must reach

@@ -844,7 +844,7 @@ def expect_op(meta, op, before, tf32_cut=False):
     """Evaluate op `op`'s contract on `before` (raw bytes in front of the op) -> Expectation."""
     tr = op["trace"]
     ref = RawMemory(meta, before)
-    ref.tf32_cut = tf32_cut and tr["kind"] == "conv" and op["label"].startswith("conv_tc")
+    ref.tf32_cut = tf32_cut and tr["kind"] == "conv" and tr["launch"]["kernel"] in ("tc2", "tc3")
     errs = run_op(ref, tr, meta) or {}
     return Expectation(meta, op, ref, errs, ref.tf32_cut)
 

@@ -319,7 +319,7 @@ def test_skipped_padding_rows_fail_only_on_poisoned_memory():
 def test_unwritten_one_row_time_tile_is_flagged():
     """T = 257 runs the 3x3 kernel in 128-row time tiles, the last one a single row: leaving it unwritten is flagged"""
     meta, blob = trace_of("ResNet34", "fp16", 1, 257)
-    i = first_op(meta, lambda tr, lab: tr["kind"] == "conv3x3" and tr["out"]["T"] == 257 and "n_mt=1" in lab)
+    i = first_op(meta, lambda tr, lab: tr["kind"] == "conv3x3" and tr["out"]["T"] == 257 and tr["launch"]["n_mt"] == 1)
     feats = np.random.default_rng(5).standard_normal((1, 257, 80))
     state = walk(meta, initial_state(meta, blob, feats), stop=i + 1)[0][i]
     tr = meta["ops"][i]["trace"]

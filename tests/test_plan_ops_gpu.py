@@ -32,7 +32,8 @@ from wespeaker_b200.models import from_synthetic  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-# (model, precision, B, T, frame counts of a masked batch or None, engine options, op kinds and label prefixes it must reach)
+# (model, precision, B, T, frame counts of a masked batch or None, engine options, op kinds, conv kernels and cluster N tiles
+# it must reach)
 CASES = {
     "ecapa1024_bf16_wide": ("ECAPA_TDNN_c1024", "bf16", 96, 200, None, {}, {"conv", "conv_tc3", "bn=256", "se_gate"}),
     "ecapa1024_bf16_T300": ("ECAPA_TDNN_c1024", "bf16", 2, 300, None, {}, {"res2_fused", "astp_fused", "scale_residual", "linear"}),
@@ -78,7 +79,7 @@ def _canonical(meta):
 
     def walk(x, key=None):
         if isinstance(x, dict):
-            return {k: walk(v, k) for k, v in x.items() if k != "label"}
+            return {k: walk(v, k) for k, v in x.items() if k not in ("label", "launch")}
         if isinstance(x, list):
             return [walk(v) for v in x]
         if isinstance(x, int) and not isinstance(x, bool) and x >= 1 << 32:
@@ -114,8 +115,12 @@ def test_plan_ops_match_contracts(case):
 
     fails, seen = [], pe.case_branches(meta["ops"], n_frames)
     for i, op in enumerate(meta["ops"]):
-        kind = op["trace"]["kind"]
-        seen |= {kind, op["label"].split()[0]} | {w for w in op["label"].split() if w.startswith("bn=")}
+        kind, g = op["trace"]["kind"], op["trace"].get("launch", {})
+        seen.add(kind)
+        if kind == "conv":
+            seen.add("conv_" + g["kernel"])
+            if g["kernel"] == "tc3":
+                seen.add(f"bn={g['bn']}")
         exp = pi.expect_op(meta, op, live, tf32_cut=prec == "tf32")
         pi.poison(exp, live)         # what the op declares written and does not read: NaN (-1 in frame counts)
         before = {a: t.clone() for a, t in live.items()}

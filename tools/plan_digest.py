@@ -13,8 +13,9 @@ activation address becomes "A<k>+<offset>" with allocations numbered in order of
 weight address becomes "W<sha256 of its fp32 source>+<offset>".  --out DIR also writes each case's canonical plan to
 DIR/<case>.json, for diffing the cases whose digests differ.  --strip-added drops the fields that later traces added before
 digesting, for comparing with builds whose traces did not name them: the optional buffers (the 3xTF32 lo twins plo, p_lo,
-W_lo, out_lo, out2_lo, the linear split-K workspace wsp and the SimAM partial sums), the kernel an op takes, tstats' eps and
-output element size, and se_gate's column sums ("kind.field": that field of that op kind only).
+W_lo, out_lo, out2_lo, the linear split-K workspace wsp and the SimAM partial sums), the kernel an op takes, the "launch"
+object (the kernel and geometry the host chose for an op), tstats' eps and output element size, and se_gate's column sums
+("kind.field": that field of that op kind only).
 """
 import argparse
 import bisect
@@ -34,7 +35,7 @@ from wespeaker_b200.models import SUPPORTED_MODELS, from_synthetic  # noqa: E402
 
 PRECISIONS = ("fp32", "tf32", "tf32x3", "bf16", "fp16")
 PLACEHOLDER = 0x7000000000   # plan_check_alloc hands out addresses from here up
-ADDED_FIELDS = ("plo", "p_lo", "W_lo", "out_lo", "out2_lo", "wsp", "partial", "kernel", "tstats.eps", "tstats.out_es",
+ADDED_FIELDS = ("plo", "p_lo", "W_lo", "out_lo", "out2_lo", "wsp", "partial", "kernel", "launch", "tstats.eps", "tstats.out_es",
                 "se_gate.colsum")
 
 

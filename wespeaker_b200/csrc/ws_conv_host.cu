@@ -21,7 +21,8 @@ static thread_local bool g_plan_check = false;
 bool plan_check_mode() { return g_plan_check; }
 PlanCheckScope::PlanCheckScope(bool on) : prev(g_plan_check) { g_plan_check = on; }
 PlanCheckScope::~PlanCheckScope() { g_plan_check = prev; }
-static std::string conv_trace(const ConvSpec& s) {
+std::string trace_of(const ConvRec& r) {
+    const ConvSpec& s = r.spec;
     std::string j = "{\"kind\":\"conv\"," + ti("es", ws_esize(s.dt)) + ",\"src\":[";
     for (int i = 0; i < s.nsrc; ++i) {
         const WsSrc& v = s.src[i];
@@ -34,13 +35,26 @@ static std::string conv_trace(const ConvSpec& s) {
         j += std::string(i ? "," : "") + "[" + std::to_string(t.src) + "," + std::to_string(t.c0) + "," + std::to_string(t.dt) + "," + std::to_string(t.df) + "," +
              std::to_string(t.wk) + "," + std::to_string(t.nch) + "]";
     }
-    const WsEpi& e = s.epi;
+    const WsEpi& e = r.tc ? r.tc->epi : r.simt->epi;
     j += "]," + tp("W", s.W) + "," + ti("Ktot", s.Ktot) + "," + ti("Cout", s.Cout) + "," + ti("B", s.B) + "," + ti("F", s.F) + "," + ti("T", s.T) +
          "," + tp("bias", e.bias) + "," + tp("rowbias", e.rowbias) + "," + ti("rowbias_ld", e.rowbias_ld) + "," + ti("act1", e.act1) + "," + tp("scale", e.scale) +
          "," + tp("shift", e.shift) + "," + tp("gate", e.gate) + "," + ti("gate_ld", e.gate_ld) + "," + ti("gate_seg", e.gate_seg) + "," + ti("gate_nseg", e.gate_nseg) + "," + tp("res", e.res) + "," + ti("res_ld", e.res_ld) + "," + ti("act2", e.act2) + "," + tp("out", e.out) +
          "," + ti("out_ld", e.out_ld) + "," + tp("out2", e.out2) + "," + ti("out2_ld", e.out2_ld) + "," + tp("add2", e.add2) + "," + ti("add2_ld", e.add2_ld) +
-         "," + tp("colsum", e.colsum) + (s.split ? tplo("W_lo", s.W_lo) + tplo("out_lo", e.out_lo) + tplo("out2_lo", e.out2_lo) : std::string()) + "}";
-    return j;
+         "," + tp("colsum", e.colsum) + (s.split ? tplo("W_lo", s.W_lo) + tplo("out_lo", e.out_lo) + tplo("out2_lo", e.out2_lo) : std::string());
+    if (!r.tc) return j + ",\"launch\":{\"kernel\":\"simt\"}}";
+    const WsTc2Params& q = *r.tc;
+    return j + ",\"launch\":{\"kernel\":\"" + (q.cl > 1 ? "tc3" : "tc2") + "\"," + ti("cl", q.cl) + "," + ti("bn", q.bn) + "," + ti("nstages", q.nstages) + "," +
+           ti("bk_bytes", q.bk_bytes) + ",\"tile\":[" + std::to_string(1 << q.bt_log2) + "," + std::to_string(1 << q.bf_log2) + "," + std::to_string(1 << q.bb_log2) + "]," +
+           ti("grid", q.grid) + "}}";
+}
+
+std::string label_of(const ConvRec& r) {
+    const ConvSpec& s = r.spec;
+    char kern[64] = "conv_simt", buf[160];
+    if (r.tc && r.tc->cl > 1) snprintf(kern, sizeof kern, "conv_tc3 cl=%d grid=%d bn=%d st=%d", r.tc->cl, r.tc->grid, r.tc->bn, r.tc->nstages);
+    else if (r.tc) snprintf(kern, sizeof kern, "conv_tc2");
+    snprintf(buf, sizeof buf, "%s pos=%lld K=%d N=%d", kern, (long long)((double)s.B * s.F * s.T), s.Ktot, s.Cout);
+    return buf;
 }
 
 void* plan_check_alloc(size_t bytes) {
@@ -377,45 +391,38 @@ static bool build_simt(const ConvSpec& s, WsSimtParams* p) {
     return true;
 }
 
-static void label_conv(PlanOp* op, const char* kern, const ConvSpec& spec) {
-    const double pos = (double)spec.B * spec.F * spec.T;
-    char buf[160];
-    snprintf(buf, sizeof buf, "%s pos=%lld K=%d N=%d", kern, (long long)pos, spec.Ktot, spec.Cout);
-    op->label = buf;
-    op->flops = 2.0 * pos * spec.Ktot * spec.Cout;
+static const char* launch_conv(const ConvRec& r, cudaStream_t s) {
+    if (r.simt) return ws_simt_launch(r.simt.get(), s);
+    return r.tc->cl > 1 ? ws_tc3_launch(r.tc.get(), s) : ws_tc2_launch(r.tc.get(), s);
 }
+
 bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
-    out->trace = [spec] { return conv_trace(spec); };
+    ConvRec rec{spec};
+    const long long pos = (long long)spec.B * spec.F * spec.T;
     const char* env_mp = getenv("WS_TC3_MIN_POS");
     const long long min_pos = env_mp ? atoll(env_mp) : 132LL * 128;   // one wave of 128-row tiles on an H100
-    if (use_tc >= 3 && (long long)spec.B * spec.F * spec.T >= min_pos) {
+    if (use_tc >= 3 && pos >= min_pos) {
         // big layers: clusters of CTAs on adjacent position tiles share the weight tile by TMA multicast
         auto q = std::make_shared<WsTc2Params>();
         // (two CTAs per cluster; WS_TC3_CL=4 takes four on the largest layers)
         const char* env_cl = getenv("WS_TC3_CL");
-        const int cl = (env_cl && atoi(env_cl) == 4 && (long long)spec.B * spec.F * spec.T >= 2LL * min_pos) ? 4 : 2;
+        const int cl = (env_cl && atoi(env_cl) == 4 && pos >= 2LL * min_pos) ? 4 : 2;
         const OpBuild r = build_tc2(spec, q.get(), cl);
-        if (r == OpBuild::built) {
-            out->run = [q](cudaStream_t s) { return ws_tc3_launch(q.get(), s); };
-            char kn[64];
-            snprintf(kn, sizeof kn, "conv_tc3 cl=%d grid=%d bn=%d st=%d", q->cl, q->grid, q->bn, q->nstages);
-            label_conv(out, kn, spec);
-            return true;
-        }
         if (r == OpBuild::error) return false;
+        if (r == OpBuild::built) rec.tc = q;
     }
-    if (use_tc >= 2) {
+    if (!rec.tc && use_tc >= 2) {
         auto q = std::make_shared<WsTc2Params>();
         if (build_tc2(spec, q.get()) != OpBuild::built) return false;
-        out->run = [q](cudaStream_t s) { return ws_tc2_launch(q.get(), s); };
-        label_conv(out, "conv_tc2", spec);
-        return true;
+        rec.tc = q;
     }
-    if (spec.epi.colsum != nullptr) { set_err("conv colsum: only the persistent tensor-core kernels (use_tc >= 2) produce column sums"); return false; }
-    auto p = std::make_shared<WsSimtParams>();
-    if (!build_simt(spec, p.get())) return false;
-    out->run = [p](cudaStream_t s) { return ws_simt_launch(p.get(), s); };
-    label_conv(out, "conv_simt", spec);
+    if (!rec.tc) {
+        if (spec.epi.colsum != nullptr) { set_err("conv colsum: only the persistent tensor-core kernels (use_tc >= 2) produce column sums"); return false; }
+        auto p = std::make_shared<WsSimtParams>();
+        if (!build_simt(spec, p.get())) return false;
+        rec.simt = p;
+    }
+    *out = plan_op(rec, launch_conv, label_of(rec), 2.0 * (double)pos * spec.Ktot * spec.Cout);
     return true;
 }
 
@@ -452,14 +459,23 @@ OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float
     q->smem_bytes = npan * 272 * 128 + 4 * w8 * 128 + npan * 256 * 128 + 1024;
     const long long units = (long long)x.B * q->ntile;
     q->grid = (int)(units < ws_num_sms() ? units : ws_num_sms());
-    op->run = [q](cudaStream_t s) { return ws_res2_launch(q.get(), s); };
-    op->trace = [=] { return "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W7", W7) + "," + tp("bias", bias) + "," +
-               tp("scale", scale) + "," + tp("shift", shift) + "," + ti("w8", w8) + "," + ti("dil", dil) + "," + tp("lens", lens) + "}"; };
-    char buf[160];
-    snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", x.B, x.T, x.C);
-    op->label = buf;
-    op->flops = 2.0 * x.B * x.T * 7.0 * 3.0 * (x.C / 8.0) * (x.C / 8.0);
+    const Res2Rec rec{q, x, out, W7};
+    *op = plan_op(rec, [](const Res2Rec& r, cudaStream_t s) { return ws_res2_launch(r.q.get(), s); }, label_of(rec),
+                  2.0 * x.B * x.T * 7.0 * 3.0 * (x.C / 8.0) * (x.C / 8.0));
     return OpBuild::built;
+}
+
+std::string trace_of(const Res2Rec& r) {
+    const WsRes2Params& q = *r.q;
+    return "{\"kind\":\"res2_fused\",\"es\":2," + tview("x", r.x) + "," + tview("out", r.out) + "," + tp("W7", r.W7) + "," + tp("bias", q.bias) + "," +
+           tp("scale", q.scale) + "," + tp("shift", q.shift) + "," + ti("w8", q.w8) + "," + ti("dil", q.dil) + "," + tp("lens", q.lens) + ",\"launch\":{" +
+           ti("ntile", q.ntile) + "," + ti("grid", q.grid) + "}}";
+}
+
+std::string label_of(const Res2Rec& r) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "res2_fused B=%d T=%d C=%d", r.x.B, r.x.T, r.x.C);
+    return buf;
 }
 
 OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats, float var_floor, PlanOp* op, const int* lens) {
@@ -502,14 +518,22 @@ OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats,
     for (int g : cand) if (nblk % g == 0 && eff(g) >= 0.92 * best) { q->g = g; break; }
     const long long units = (long long)x.B * (nblk / q->g);
     q->grid = (int)(units < sms ? units : sms);
-    op->run = [q](cudaStream_t s) { return ws_astp_launch(q.get(), s); };
-    op->trace = [=] { return "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", x) + "," + tview("h", h) + "," + tp("W2", W2) + "," + tp("stats", stats) + "," +
-               tp("lens", lens) + "," + tf("eps", var_floor) + "}"; };
-    char buf[160];
-    snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", x.B, x.T, x.C, q->g, q->grid);
-    op->label = buf;
-    op->flops = 2.0 * x.B * x.T * 128.0 * x.C;
+    const AstpRec rec{q, x, h, W2};
+    *op = plan_op(rec, [](const AstpRec& r, cudaStream_t s) { return ws_astp_launch(r.q.get(), s); }, label_of(rec),
+                  2.0 * x.B * x.T * 128.0 * x.C);
     return OpBuild::built;
+}
+
+std::string trace_of(const AstpRec& r) {
+    const WsAstpParams& q = *r.q;
+    return "{\"kind\":\"astp_fused\",\"es\":2," + tview("x", r.x) + "," + tview("h", r.h) + "," + tp("W2", r.W2) + "," + tp("stats", q.out) + "," +
+           tp("lens", q.lens) + "," + tf("eps", q.var_floor) + ",\"launch\":{" + ti("g", q.g) + "," + ti("grid", q.grid) + "}}";
+}
+
+std::string label_of(const AstpRec& r) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "astp_fused B=%d T=%d C=%d g=%d grid=%d", r.q->B, r.q->T, r.q->C, r.q->g, r.q->grid);
+    return buf;
 }
 
 OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
@@ -635,17 +659,26 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
     q->bias = bias;
     q->relu = relu;   // 0 none, 1 ReLU, 2 Hardtanh(0, 20)
     q->lens = lens;
-    char buf[200];
-    snprintf(buf, sizeof buf, "conv3x3 B=%d F=%d T=%d Cin=%d Cout=%d s=%dx%d caseB=%d nb=%d n_mt=%d R=%d res=%d", q->B, q->F, q->T,
-             q->Cin, q->Cout, q->sf, q->st, q->case_b, q->nb, q->n_mt, q->R, q->res != nullptr);
-    op->label = buf;
-    op->flops = 2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout;
-    const bool has_res = res != nullptr;
-    const View rv = has_res ? *res : View();
-    op->trace = [=] { return "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", x) + "," + tview("out", out) + "," + tp("W", W) + "," + tp("bias", bias) + "," +
-               (has_res ? tview("res", rv) : std::string("\"res\":null")) + "," + ti("relu", relu) + "," + ti("sf", stride_f) + "," + ti("st", stride_t) + "," + tp("lens", lens) + "}"; };
-    op->run = [q](cudaStream_t s) { return ws_c3_launch(q.get(), s); };
+    const Conv3x3Rec rec{q, x, out, res ? *res : View(), W};
+    *op = plan_op(rec, [](const Conv3x3Rec& r, cudaStream_t s) { return ws_c3_launch(r.q.get(), s); }, label_of(rec),
+                  2.0 * q->B * q->F * q->T * 9.0 * q->Cin * q->Cout);
     return OpBuild::built;
+}
+
+std::string trace_of(const Conv3x3Rec& r) {
+    const WsC3Params& q = *r.q;
+    return "{\"kind\":\"conv3x3\",\"es\":2," + tview("x", r.x) + "," + tview("out", r.out) + "," + tp("W", r.W) + "," + tp("bias", q.bias) + "," +
+           (q.res ? tview("res", r.res) : std::string("\"res\":null")) + "," + ti("relu", q.relu) + "," + ti("sf", q.sf) + "," + ti("st", q.st) + "," + tp("lens", q.lens) +
+           ",\"launch\":{" + ti("case_b", q.case_b) + "," + ti("nb", q.nb) + "," + ti("n_mt", q.n_mt) + "," + ti("tb", q.tb) + "," + ti("n_tt", q.n_tt) + "," + ti("R", q.R) + "," +
+           ti("stg_bufs", q.stg_bufs) + "," + ti("w_resident", q.w_resident) + "," + ti("grid", q.grid) + "}}";
+}
+
+std::string label_of(const Conv3x3Rec& r) {
+    const WsC3Params& q = *r.q;
+    char buf[200];
+    snprintf(buf, sizeof buf, "conv3x3 B=%d F=%d T=%d Cin=%d Cout=%d s=%dx%d caseB=%d nb=%d n_mt=%d R=%d res=%d", q.B, q.F, q.T, q.Cin, q.Cout, q.sf, q.st,
+             q.case_b, q.nb, q.n_mt, q.R, q.res != nullptr);
+    return buf;
 }
 
 extern "C" int ws_cam_smem_bytes(int nmt, int nstages);
@@ -694,25 +727,28 @@ OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std
     cuuint32_t boxx[3] = {64, 128, 1}, boxo[3] = {32, 128, 1};
     if (!encode_map(&q->xmap, X.dt, X.p, 3, dims, str, boxx, 128)) return OpBuild::error;
     if (!encode_map(&q->omap, X.dt, X.p, 3, dims, str, boxo, 64)) return OpBuild::error;
-    char buf[160];
-    snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", l0, l1 - 1, X.B, X.T);
-    op->label = buf;
-    op->run = [q](cudaStream_t s) { return ws_cam_launch(q.get(), s); };
-    // layers [l0, l1) over the concat buffer, each with what its descriptor points at
-    const std::vector<WsCamLayer> ls(layers.begin() + l0, layers.begin() + l1);
-    const std::vector<std::array<const void*, 2>> lw(weights.begin() + l0, weights.begin() + l1);
-    op->trace = [=] {
-        std::string j = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(X.dt)) + "," + tview("X", X) + "," + tp("lens", lens) + "," +
-                         ti("seg_len", q->seg_len) + ",\"layers\":[";
-        for (size_t k = 0; k < ls.size(); ++k) {
-            const WsCamLayer& L = ls[k];
-            j += std::string(k ? "," : "") + "{" + tp("W1", lw[k][0]) + "," + tp("Wl", lw[k][1]) + "," + tp("bn1_scale", L.bn1_scale) + "," +
-                 tp("bn1_shift", L.bn1_shift) + "," + tp("bias2", L.bias2) + "," + tp("w1c_t", L.w1c_t) + "," + tp("b1c", L.b1c) + "," +
-                 tp("w2c_t", L.w2c_t) + "," + tp("b2c", L.b2c) + "," + ti("cin", L.cin) + "," + ti("dil", L.dil) + "}";
-        }
-        return j + "]}";
-    };
+    const CamRec rec{q, X, {layers.begin() + l0, layers.begin() + l1}, {weights.begin() + l0, weights.begin() + l1}};
+    *op = plan_op(rec, [](const CamRec& r, cudaStream_t s) { return ws_cam_launch(r.q.get(), s); }, label_of(rec));
     return OpBuild::built;
+}
+
+std::string trace_of(const CamRec& r) {   // layers [l0, l1) over the concat buffer, each with what its descriptor points at
+    const WsCamParams& q = *r.q;
+    std::string j = "{\"kind\":\"cam_dense\"," + ti("es", ws_esize(q.dtype)) + "," + tview("X", r.X) + "," + tp("lens", q.lens) + "," + ti("seg_len", q.seg_len) +
+                    ",\"layers\":[";
+    for (size_t k = 0; k < r.layers.size(); ++k) {
+        const WsCamLayer& L = r.layers[k];
+        j += std::string(k ? "," : "") + "{" + tp("W1", r.weights[k][0]) + "," + tp("Wl", r.weights[k][1]) + "," + tp("bn1_scale", L.bn1_scale) + "," +
+             tp("bn1_shift", L.bn1_shift) + "," + tp("bias2", L.bias2) + "," + tp("w1c_t", L.w1c_t) + "," + tp("b1c", L.b1c) + "," +
+             tp("w2c_t", L.w2c_t) + "," + tp("b2c", L.b2c) + "," + ti("cin", L.cin) + "," + ti("dil", L.dil) + "}";
+    }
+    return j + "],\"launch\":{" + ti("nmt", q.nmt) + "," + ti("nstages", q.nstages) + "," + ti("grid", q.grid) + "}}";
+}
+
+std::string label_of(const CamRec& r) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "cam_dense layers %d..%d B=%d T=%d", r.q->l0, r.q->l1 - 1, r.q->B, r.q->T);
+    return buf;
 }
 
 }  // namespace ws

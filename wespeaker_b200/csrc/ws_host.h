@@ -7,6 +7,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -97,21 +98,23 @@ inline std::string tview(const char* n, const View& v) {
     return std::string("\"") + n + "\":{" + tp("p", v.p) + tplo("plo", v.plo) + "," + ti("B", v.B) + "," + ti("F", v.F) + "," + ti("T", v.T) + "," + ti("C", v.C) + "," + ti("ld", v.ld) + "}";
 }
 inline std::string tes(int dt) { return ti("es", ws_esize(dt)); }
+// the kernel a bandwidth op takes (tstats, linear, astp_stats): in "launch", like every host choice, and at the top level,
+// where earlier traces named it
+inline std::string tkernel(const char* k) { return std::string(",\"kernel\":\"") + k + "\",\"launch\":{\"kernel\":\"" + k + "\"}"; }
 
 // The plan trace of each bandwidth op, from the record its launcher takes (ws_kernels.cuh)
 inline std::string trace_of(const WsConvert& a) { return "{\"kind\":\"convert\"," + tes(a.dt) + "," + tp("in", a.in) + "," + tp("out", a.out) + "," + ti("n", a.n) + tplo("out_lo", a.lo) + "}"; }
 inline std::string trace_of(const WsTstats& a) {
     static const char* kern[] = {"scalar", "tmean8", "tstats8"};
     return "{\"kind\":\"tstats\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("pre_scale", a.pre_scale) + "," + tp("pre_shift", a.pre_shift) + "," + tp("out", a.out) + "," +
-           ti("out_es", ws_esize(a.odt)) + "," + ti("out_ld", a.out_ld) + "," + ti("std_off", a.std_off) + "," + tff("eps", a.eps) + "," + tp("lens", a.lens) + ",\"kernel\":\"" + kern[a.kernel] +
-           "\"}";
+           ti("out_es", ws_esize(a.odt)) + "," + ti("out_ld", a.out_ld) + "," + ti("std_off", a.std_off) + "," + tff("eps", a.eps) + "," + tp("lens", a.lens) + tkernel(kern[a.kernel]) + "}";
 }
 inline std::string trace_of(const WsZeroTail& a) { return "{\"kind\":\"zero_tail\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("lens", a.lens) + "}"; }
 inline std::string trace_of(const WsLensDerive& a) { return "{\"kind\":\"lens_derive\"," + tp("lens", a.lens) + "," + ti("B", a.B) + "," + ti("T", a.T) + "," + ti("levels", a.levels) + "}"; }
 inline std::string trace_of(const WsLinear& a) {
     return "{\"kind\":\"linear\"," + tp("in", a.in) + "," + ti("in_ld", a.in_ld) + "," + tp("in2", a.in2) + "," + ti("in2_ld", a.in2_ld) + "," + ti("rows_per_b", a.rows_per_b) + "," + tp("W", a.W) +
            "," + tp("bias", a.bias) + "," + tp("out", a.out) + "," + ti("out_ld", a.out_ld) + "," + ti("R", a.R) + "," + ti("I", a.I) + "," + ti("O", a.O) + "," + ti("act", a.act) + tplo("wsp", a.wsp) +
-           ",\"kernel\":\"" + (a.kernel == WS_LINEAR_ROWS64 ? "rows64" : "rows16") + "\"}";
+           tkernel(a.kernel == WS_LINEAR_ROWS64 ? "rows64" : "rows16") + "}";
 }
 inline std::string trace_of(const WsScaleResidual& a) {
     return "{\"kind\":\"scale_residual\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tp("gate", a.gate) + "," + tview("res", a.res) + "," + tview("out", a.out) + "}";
@@ -121,7 +124,7 @@ inline std::string trace_of(const WsAffCombine& a) {
 }
 inline std::string trace_of(const WsAstpStats& a) {
     return "{\"kind\":\"astp_stats\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + tview("logits", a.logits) + "," + tp("stats", a.stats) + "," + tp("lens", a.lens) + "," + tff("eps", a.var_floor) +
-           ",\"kernel\":\"" + (a.kernel == WS_ASTP_STATS4 ? "stats4" : "scalar") + "\"}";
+           tkernel(a.kernel == WS_ASTP_STATS4 ? "stats4" : "scalar") + "}";
 }
 inline std::string trace_of(const WsSimamStats& a) {
     return "{\"kind\":\"simam_stats\"," + tes(a.y.dt) + "," + tview("x", a.y) + "," + tp("stats", a.stats) + "," + tp("lens", a.lens) + tplo("partial", a.partial) + "}";
@@ -152,6 +155,53 @@ inline std::string trace_of(const WsSeGate& a) {
 inline std::string trace_of(const WsCamGate& a) {
     return "{\"kind\":\"cam_gate\"," + tes(a.x.dt) + "," + tview("x", a.x) + "," + ti("seg_len", a.seg_len) + "," + tp("W1", a.W1) + "," + tp("b1", a.b1) + "," + tp("W2", a.W2) + "," + tp("b2", a.b2) +
            "," + ti("H", a.H) + "," + ti("G", a.G) + "," + tp("gate", a.gate) + "}";
+}
+
+// The tensor-core ops, one record each: the parameter block its launcher reads, and the operands its tensor maps were encoded
+// from (a CUtensorMap cannot be read back).  trace_of writes the op's contract - every scalar the kernel reads taken from the
+// parameter block - plus a "launch" object with the kernel and geometry the host chose, which may depend on the device (SM
+// count, co-resident clusters); label_of writes the op's label.
+struct ConvRec {                               // the conv-GEMM: tc (tc3 when tc->cl > 1, else tc2) or simt
+    ConvSpec spec;                             // source views, taps and weights
+    std::shared_ptr<const WsTc2Params> tc;
+    std::shared_ptr<const WsSimtParams> simt;
+};
+struct Conv3x3Rec {
+    std::shared_ptr<const WsC3Params> q;
+    View x, out, res;                          // res: meaningful where q->res is set
+    const void* W;
+};
+struct Res2Rec {
+    std::shared_ptr<const WsRes2Params> q;
+    View x, out;
+    const void* W7;
+};
+struct AstpRec {
+    std::shared_ptr<const WsAstpParams> q;
+    View x, h;
+    const void* W2;
+};
+struct CamRec {
+    std::shared_ptr<const WsCamParams> q;
+    View X;
+    std::vector<WsCamLayer> layers;                      // host copies of the descriptors of layers [q->l0, q->l1)
+    std::vector<std::array<const void*, 2>> weights;     // the (W1, Wl) each one's tensor maps were encoded from
+};
+std::string trace_of(const ConvRec& r);
+std::string trace_of(const Conv3x3Rec& r);
+std::string trace_of(const Res2Rec& r);
+std::string trace_of(const AstpRec& r);
+std::string trace_of(const CamRec& r);
+std::string label_of(const ConvRec& r);
+std::string label_of(const Conv3x3Rec& r);
+std::string label_of(const Res2Rec& r);
+std::string label_of(const AstpRec& r);
+std::string label_of(const CamRec& r);
+
+// A plan op launched and traced from one record: launch(rec, stream) runs it, trace_of(rec) describes it
+template <class Rec, class Launch>
+PlanOp plan_op(const Rec& rec, Launch launch, std::string label, double flops = 0) {
+    return PlanOp{[rec, launch](cudaStream_t s) { return launch(rec, s); }, std::move(label), flops, [rec] { return trace_of(rec); }};
 }
 
 // Build a launch closure for `spec`; use_tc selects a tensor-core kernel (needs dt-aligned shapes) else FFMA.

@@ -305,7 +305,7 @@ struct Builder {
     // a bandwidth op: its argument record, which both its launch and its plan trace (trace_of, ws_host.h) read
     template <class Rec>
     void push(const Rec& a, const char* (*launch)(const Rec&, cudaStream_t), const char* label) {
-        push(PlanOp{[a, launch](cudaStream_t s) { return launch(a, s); }, label, 0.0, [a] { return trace_of(a); }});
+        push(plan_op(a, launch, label));
     }
     // length-masked plans: frame counts of stride level k (nullptr in ordinary plans), and "zero the rows behind every
     // utterance's end" for tensors a time-mixing op is about to read (the reference's unpadded forward sees zero padding)
