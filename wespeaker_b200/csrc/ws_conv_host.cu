@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <mutex>
 
@@ -197,6 +198,36 @@ static bool encode_map(CUtensorMap* m, int dt, const void* ptr, int rank, const 
     return true;
 }
 
+// A tensor map from its extents, strides in elements (the innermost stride is 1) and box, all innermost first; the rank is
+// the number of extents.
+static bool encode_strided(CUtensorMap* m, int dt, const void* ptr, std::initializer_list<long long> dims,
+                           std::initializer_list<long long> strides, std::initializer_list<int> box, int swizzle_bytes) {
+    const int rank = (int)dims.size();
+    if (rank < 1 || rank > 5 || (int)strides.size() != rank - 1 || (int)box.size() != rank) {
+        set_err("tensor map: extents, strides and box disagree in rank");
+        return false;
+    }
+    cuuint64_t d[5], s[4];
+    cuuint32_t b[5];
+    for (int i = 0; i < rank; ++i) { d[i] = (cuuint64_t)dims.begin()[i]; b[i] = (cuuint32_t)box.begin()[i]; }
+    for (int i = 0; i + 1 < rank; ++i) s[i] = (cuuint64_t)strides.begin()[i] * ws_esize(dt);
+    return encode_map(m, dt, ptr, rank, d, s, b, swizzle_bytes);
+}
+
+// A channels-last view: rank 4 over (C, T, F, B), or rank 3 over (C, T, B) for a view with F == 1, as the box's rank says
+static bool encode_view(CUtensorMap* m, const View& v, std::initializer_list<int> box, int swizzle_bytes) {
+    if (box.size() == 4)
+        return encode_strided(m, v.dt, v.p, {v.C, v.T, v.F, v.B}, {v.ld, v.T * v.ld, (long long)v.F * v.T * v.ld}, box, swizzle_bytes);
+    if (v.F != 1) { set_err("tensor map: a rank-3 view map needs F == 1"); return false; }
+    return encode_strided(m, v.dt, v.p, {v.C, v.T, v.B}, {v.ld, v.T * v.ld}, box, swizzle_bytes);
+}
+
+// A row-major rows x cols matrix (row pitch cols), such as a [Cout][K] weight
+static bool encode_matrix(CUtensorMap* m, int dt, const void* ptr, long long cols, long long rows, std::initializer_list<int> box,
+                          int swizzle_bytes) {
+    return encode_strided(m, dt, ptr, {cols, rows}, {cols}, box, swizzle_bytes);
+}
+
 static int ilog2(int v) {
     int l = 0;
     while ((1 << l) < v) ++l;
@@ -245,19 +276,14 @@ static bool tc2_geometry(const ConvSpec& s, WsTc2Params* q) {
     q->B = B; q->F = F; q->T = T;
     // ---- activation maps, one per source view (unused slots repeat the first)
     for (int i = 0; i < s.nsrc; ++i) {
-        const WsSrc& v = s.src[i];
-        cuuint64_t dims[4], str[3];
-        if (flat) {
-            dims[0] = (cuuint64_t)v.C; dims[1] = (cuuint64_t)T; dims[2] = 1; dims[3] = 1;
-            str[0] = (cuuint64_t)v.sT * es; str[1] = (cuuint64_t)T * v.sT * es; str[2] = str[1];
-        } else {
-            dims[0] = (cuuint64_t)v.C; dims[1] = (cuuint64_t)v.T; dims[2] = (cuuint64_t)v.F; dims[3] = (cuuint64_t)v.B;
-            str[0] = (cuuint64_t)v.sT * es; str[1] = (cuuint64_t)v.sF * es; str[2] = (cuuint64_t)v.sB * es;
-        }
-        cuuint32_t box[4] = {(cuuint32_t)bk_elems, (cuuint32_t)bt, (cuuint32_t)bf, (cuuint32_t)bb};
-        if (!encode_map(&q->amap[i], s.dt, v.ptr, 4, dims, str, box, q->bk_bytes)) return false;
+        WsSrc v = s.src[i];
+        if (flat) { v.B = 1; v.F = 1; v.T = T; v.sF = v.sB = T * v.sT; }   // all positions as one row
+        auto enc = [&](CUtensorMap* m, const void* p) {
+            return encode_strided(m, s.dt, p, {v.C, v.T, v.F, v.B}, {v.sT, v.sF, v.sB}, {bk_elems, bt, bf, bb}, q->bk_bytes);
+        };
+        if (!enc(&q->amap[i], v.ptr)) return false;
         q->amap_lo[i] = q->amap[i];
-        if (s.split && !encode_map(&q->amap_lo[i], s.dt, v.ptr_lo, 4, dims, str, box, q->bk_bytes)) return false;
+        if (s.split && !enc(&q->amap_lo[i], v.ptr_lo)) return false;
     }
     for (int i = s.nsrc; i < WS_MAX_SRC; ++i) { q->amap[i] = q->amap[0]; q->amap_lo[i] = q->amap_lo[0]; }
     return true;
@@ -335,28 +361,15 @@ static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
     q->panel_bytes = bn * es >= 128 ? 128 : bn * es;
     const int panel_cols = q->panel_bytes / es;
     const int bk_elems = q->bk_bytes / es;
-    {   // weights map with the chosen N tile
-        cuuint64_t dims[2] = {(cuuint64_t)s.Ktot, (cuuint64_t)s.Cout};
-        cuuint64_t str[1] = {(cuuint64_t)s.Ktot * es};
-        cuuint32_t box[2] = {(cuuint32_t)bk_elems, (cuuint32_t)(bn / cl)};   // the rows ONE CTA loads per k-block
-        if (!encode_map(&q->wmap, s.dt, s.W, 2, dims, str, box, q->bk_bytes)) return OpBuild::error;
-        q->wmap_lo = q->wmap;
-        if (s.split && !encode_map(&q->wmap_lo, s.dt, s.W_lo, 2, dims, str, box, q->bk_bytes)) return OpBuild::error;
-    }
-    // output / epilogue-input maps: same tile geometry as the A maps over the output positions
-    const bool flat = s.dense_pointwise;
-    auto out_map = [&](CUtensorMap* m, const void* ptr, long long ld) -> bool {
-        cuuint64_t dims[4], str[3];
-        cuuint32_t box[4] = {(cuuint32_t)panel_cols, (cuuint32_t)(1 << q->bt_log2), (cuuint32_t)(1 << q->bf_log2),
-                             (cuuint32_t)(1 << q->bb_log2)};
-        if (flat) {
-            dims[0] = (cuuint64_t)s.Cout; dims[1] = (cuuint64_t)q->T; dims[2] = 1; dims[3] = 1;
-            str[0] = (cuuint64_t)ld * es; str[1] = (cuuint64_t)q->T * ld * es; str[2] = str[1];
-        } else {
-            dims[0] = (cuuint64_t)s.Cout; dims[1] = (cuuint64_t)s.T; dims[2] = (cuuint64_t)s.F; dims[3] = (cuuint64_t)s.B;
-            str[0] = (cuuint64_t)ld * es; str[1] = (cuuint64_t)s.T * ld * es; str[2] = (cuuint64_t)s.F * s.T * ld * es;
-        }
-        return encode_map(m, s.dt, ptr, 4, dims, str, box, q->panel_bytes);
+    // weights map with the chosen N tile: box of the rows ONE CTA loads per k-block
+    if (!encode_matrix(&q->wmap, s.dt, s.W, s.Ktot, s.Cout, {bk_elems, bn / cl}, q->bk_bytes)) return OpBuild::error;
+    q->wmap_lo = q->wmap;
+    if (s.split && !encode_matrix(&q->wmap_lo, s.dt, s.W_lo, s.Ktot, s.Cout, {bk_elems, bn / cl}, q->bk_bytes)) return OpBuild::error;
+    // output / epilogue-input maps: same tile geometry as the A maps over the output positions (q's extents: one row of
+    // all positions for a dense 1x1 conv)
+    auto out_map = [&](CUtensorMap* m, const void* ptr, long long ld) {
+        const View o{const_cast<void*>(ptr), nullptr, q->B, q->F, q->T, s.Cout, ld, s.dt};
+        return encode_view(m, o, {panel_cols, 1 << q->bt_log2, 1 << q->bf_log2, 1 << q->bb_log2}, q->panel_bytes);
     };
     int oi = 0;
     if (!out_map(&q->omap[oi++], e.out, e.out_ld)) return OpBuild::error;
@@ -429,30 +442,14 @@ bool make_conv_op(const ConvSpec& spec, int use_tc, PlanOp* out) {
 OpBuild make_res2_op(const View& x, const View& out, const void* W7, const float* bias, const float* scale,
                      const float* shift, int w8, int dil, PlanOp* op, const int* lens) {
     // T > 256: time tiles with a 32-row halo per side cover the chain's receptive field (7 * dil rows) up to dilation 4
-    if (x.dt == WS_F32 || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7)
+    if (x.dt == WS_F32 || out.dt != x.dt || (w8 != 64 && w8 != 128) || (x.T > 256 && dil > 4) || x.F != 1 || dil < 1 || dil > 7)
         return OpBuild::outside;
     auto q = std::make_shared<WsRes2Params>();
     memset(q.get(), 0, sizeof(WsRes2Params));
-    auto act_map = [&](CUtensorMap* m, const View& v) {
-        cuuint64_t dims[3] = {(cuuint64_t)v.C, (cuuint64_t)v.T, (cuuint64_t)v.B};
-        cuuint64_t str[2] = {(cuuint64_t)v.ld * 2, (cuuint64_t)v.T * v.ld * 2};
-        cuuint32_t box[3] = {64, 128, 1};
-        return encode_map(m, v.dt, v.p, 3, dims, str, box, 128);
-    };
-    if (!act_map(&q->xmap, x) || !act_map(&q->omap, out)) return OpBuild::error;
-    {
-        cuuint64_t dims[3] = {(cuuint64_t)out.C, (cuuint64_t)out.T, (cuuint64_t)out.B};
-        cuuint64_t str[2] = {(cuuint64_t)out.ld * 2, (cuuint64_t)out.T * out.ld * 2};
-        cuuint32_t box[3] = {64, 64, 1};
-        if (!encode_map(&q->omap64, out.dt, out.p, 3, dims, str, box, 128)) return OpBuild::error;
-    }
+    if (!encode_view(&q->xmap, x, {64, 128, 1}, 128) || !encode_view(&q->omap, out, {64, 128, 1}, 128) ||
+        !encode_view(&q->omap64, out, {64, 64, 1}, 128) || !encode_matrix(&q->wmap, x.dt, W7, 3 * w8, 7 * w8, {64, w8}, 128))
+        return OpBuild::error;
     q->ntile = x.T <= 256 ? 1 : (x.T + 191) / 192;
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)(3 * w8), (cuuint64_t)(7 * w8)};
-        cuuint64_t str[1] = {(cuuint64_t)(3 * w8) * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)w8};
-        if (!encode_map(&q->wmap, x.dt, W7, 2, dims, str, box, 128)) return OpBuild::error;
-    }
     q->x = x.p; q->ld = x.ld; q->bias = bias; q->scale = scale; q->shift = shift; q->lens = lens;
     q->B = x.B; q->T = x.T; q->w8 = w8; q->dil = dil; q->dtype = x.dt;
     const int npan = w8 / 64;
@@ -484,24 +481,9 @@ OpBuild make_astp_op(const View& x, const View& h, const void* W2, float* stats,
         return OpBuild::outside;
     auto q = std::make_shared<WsAstpParams>();
     memset(q.get(), 0, sizeof(WsAstpParams));
-    {
-        cuuint64_t dims[3] = {128, (cuuint64_t)h.T, (cuuint64_t)h.B};
-        cuuint64_t str[2] = {128 * 2, (cuuint64_t)h.T * 128 * 2};
-        cuuint32_t box[3] = {64, 256, 1};
-        if (!encode_map(&q->hmap, h.dt, h.p, 3, dims, str, box, 128)) return OpBuild::error;
-    }
-    {
-        cuuint64_t dims[2] = {128, (cuuint64_t)x.C};
-        cuuint64_t str[1] = {128 * 2};
-        cuuint32_t box[2] = {64, 128};
-        if (!encode_map(&q->wmap, x.dt, W2, 2, dims, str, box, 128)) return OpBuild::error;
-    }
-    {
-        cuuint64_t dims[3] = {(cuuint64_t)x.C, (cuuint64_t)x.T, (cuuint64_t)x.B};
-        cuuint64_t str[2] = {(cuuint64_t)x.ld * 2, (cuuint64_t)x.T * x.ld * 2};
-        cuuint32_t box[3] = {128, 128, 1};
-        if (!encode_map(&q->xmap, x.dt, x.p, 3, dims, str, box, 0)) return OpBuild::error;
-    }
+    if (!encode_view(&q->hmap, h, {64, 256, 1}, 128) || !encode_matrix(&q->wmap, x.dt, W2, 128, x.C, {64, 128}, 128) ||
+        !encode_view(&q->xmap, x, {128, 128, 1}, 0))
+        return OpBuild::error;
     q->x = x.p; q->x_ld = x.ld; q->out = stats; q->B = x.B; q->T = x.T; q->C = x.C; q->dtype = x.dt; q->lens = lens;
     q->var_floor = var_floor;
     // channel blocks per unit: the largest g whose static round-robin over the SMs stays within 8 % of the best balance
@@ -538,18 +520,18 @@ std::string label_of(const AstpRec& r) {
 
 OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const float* bias, const View* res, int relu,
                         PlanOp* op, int stride_f, int stride_t, const int* lens) {
-    const int Cin = x.C, Cout = out.C, Tin = x.T, Fin = x.F, B = x.B;
+    const int Cin = x.C, Cout = out.C, Tin = x.T, Fin = x.F, B = x.B, es = ws_esize(x.dt);
     const int F = (Fin + 2 - 3) / stride_f + 1, T = (Tin + 2 - 3) / stride_t + 1;   // output extents
     auto chan_ok = [](int c) { return c == 32 || c == 64 || c == 128; };
-    if (x.dt == WS_F32 || out.dt != x.dt || !chan_ok(Cin) || !chan_ok(Cout) || out.B != B || out.F != F || out.T != T ||
-        (stride_f != 1 && stride_f != 2) || (stride_t != 1 && stride_t != 2) || T < 1 || F < 1 || (x.ld * 2) % 16 != 0 || (out.ld * 2) % 16 != 0 || (res && (res->ld * 2) % 16 != 0))
+    if (x.dt == WS_F32 || out.dt != x.dt || (res && res->dt != x.dt) || !chan_ok(Cin) || !chan_ok(Cout) || out.B != B || out.F != F || out.T != T ||
+        (stride_f != 1 && stride_f != 2) || (stride_t != 1 && stride_t != 2) || T < 1 || F < 1 || (x.ld * es) % 16 != 0 || (out.ld * es) % 16 != 0 || (res && (res->ld * es) % 16 != 0))
         return OpBuild::outside;
     auto q = std::make_shared<WsC3Params>();
     memset(q.get(), 0, sizeof(WsC3Params));
     q->B = B; q->F = F; q->T = T; q->Cin = Cin; q->Cout = Cout; q->dtype = x.dt;
     q->sf = stride_f; q->st = stride_t;
-    q->row_bytes = Cin * 2 >= 128 ? 128 : Cin * 2;
-    q->kc = q->row_bytes / 2;
+    q->row_bytes = Cin * es >= 128 ? 128 : Cin * es;
+    q->kc = q->row_bytes / es;
     q->npan = Cin / q->kc;
     q->N = Cout; q->n_nt = 1;
     // ---- geometry of one ring slot / one step: first candidate whose ring (>= 4 slots) fits in shared memory
@@ -583,7 +565,7 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
         // warp sets its own unit
         q->panel_cols = std::min(64, q->N);
         if (q->panel_cols == 64 && n_mt * (q->N / 64) < 2) q->panel_cols = 32;
-        q->panel_bytes = q->panel_cols * 2;
+        q->panel_bytes = q->panel_cols * es;
         q->stg_rows = case_b ? 136 : 128;
         const int slot_bytes = q->npan * q->slot_rows * q->row_bytes;
         const int wblk = q->N * q->row_bytes, nwblk = 9 * q->npan;
@@ -620,39 +602,25 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
     q->grid = q->total_steps < sms ? q->total_steps : sms;
     // ---- tensor maps
     if (stride_t == 2) {   // even / odd time planes of the input as two tensors with a doubled t stride
-        cuuint64_t str[3] = {(cuuint64_t)x.ld * 4, (cuuint64_t)Tin * x.ld * 2, (cuuint64_t)Fin * Tin * x.ld * 2};
-        cuuint64_t de[4] = {(cuuint64_t)Cin, (cuuint64_t)((Tin + 1) / 2), (cuuint64_t)Fin, (cuuint64_t)B};
-        cuuint64_t dod[4] = {(cuuint64_t)Cin, (cuuint64_t)std::max(1, Tin / 2), (cuuint64_t)Fin, (cuuint64_t)B};
-        cuuint32_t be[4] = {(cuuint32_t)q->kc, (cuuint32_t)q->tb, 1, 1}, bo[4] = {(cuuint32_t)q->kc, (cuuint32_t)(q->tb + 1), 1, 1};
         if (Tin < 2) return OpBuild::outside;
-        if (!encode_map(&q->amap, x.dt, x.p, 4, de, str, be, q->row_bytes)) return OpBuild::error;
-        if (!encode_map(&q->amap_tail, x.dt, (const char*)x.p + (size_t)x.ld * 2, 4, dod, str, bo, q->row_bytes)) return OpBuild::error;
+        const long long sF = Tin * x.ld, sB = Fin * sF;
+        if (!encode_strided(&q->amap, x.dt, x.p, {Cin, (Tin + 1) / 2, Fin, B}, {2 * x.ld, sF, sB}, {q->kc, q->tb, 1, 1}, q->row_bytes) ||
+            !encode_strided(&q->amap_tail, x.dt, (const char*)x.p + x.ld * es, {Cin, std::max(1, Tin / 2), Fin, B}, {2 * x.ld, sF, sB},
+                            {q->kc, q->tb + 1, 1, 1}, q->row_bytes))
+            return OpBuild::error;
     } else {
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Tin, (cuuint64_t)Fin, (cuuint64_t)B};
-        cuuint64_t str[3] = {(cuuint64_t)x.ld * 2, (cuuint64_t)Tin * x.ld * 2, (cuuint64_t)Fin * Tin * x.ld * 2};
-        cuuint32_t box[4] = {(cuuint32_t)q->kc, (cuuint32_t)(q->single_box ? q->P : 128), 1, (cuuint32_t)q->nb};
-        if (!encode_map(&q->amap, x.dt, x.p, 4, dims, str, box, q->row_bytes)) return OpBuild::error;
-        cuuint32_t boxt[4] = {(cuuint32_t)q->kc, 2, 1, 1};
-        if (!encode_map(&q->amap_tail, x.dt, x.p, 4, dims, str, boxt, q->row_bytes)) return OpBuild::error;
+        if (!encode_view(&q->amap, x, {q->kc, q->single_box ? q->P : 128, 1, q->nb}, q->row_bytes) ||
+            !encode_view(&q->amap_tail, x, {q->kc, 2, 1, 1}, q->row_bytes))
+            return OpBuild::error;
     }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)(9 * Cin), (cuuint64_t)Cout};
-        cuuint64_t str[1] = {(cuuint64_t)(9 * Cin) * 2};
-        cuuint32_t box[2] = {(cuuint32_t)q->kc, (cuuint32_t)q->N};
-        if (!encode_map(&q->wmap, x.dt, W, 2, dims, str, box, q->row_bytes)) return OpBuild::error;
-    }
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)F, (cuuint64_t)B};
-        cuuint64_t str[3] = {(cuuint64_t)out.ld * 2, (cuuint64_t)T * out.ld * 2, (cuuint64_t)F * T * out.ld * 2};
-        cuuint32_t box[4] = {(cuuint32_t)q->panel_cols, (cuuint32_t)(q->case_b ? q->P : 128), 1, (cuuint32_t)(q->case_b ? q->nb : 1)};
-        if (!encode_map(&q->omap, x.dt, out.p, 4, dims, str, box, q->panel_bytes)) return OpBuild::error;
-    }
+    const std::initializer_list<int> obox = {q->panel_cols, q->case_b ? q->P : 128, 1, q->case_b ? q->nb : 1};
+    if (!encode_matrix(&q->wmap, x.dt, W, 9 * Cin, Cout, {q->kc, q->N}, q->row_bytes) || !encode_view(&q->omap, out, obox, q->panel_bytes))
+        return OpBuild::error;
     q->rmap = q->omap;
-    if (res) {
-        cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)T, (cuuint64_t)F, (cuuint64_t)B};
-        cuuint64_t str[3] = {(cuuint64_t)res->ld * 2, (cuuint64_t)T * res->ld * 2, (cuuint64_t)F * T * res->ld * 2};
-        cuuint32_t box[4] = {(cuuint32_t)q->panel_cols, (cuuint32_t)(q->case_b ? q->P : 128), 1, (cuuint32_t)(q->case_b ? q->nb : 1)};
-        if (!encode_map(&q->rmap, x.dt, res->p, 4, dims, str, box, q->panel_bytes)) return OpBuild::error;
+    if (res) {   // the residual over out's extents, at its own row pitch
+        View r = out;
+        r.p = res->p; r.ld = res->ld;
+        if (!encode_view(&q->rmap, r, obox, q->panel_bytes)) return OpBuild::error;
     }
     q->res = res ? res->p : nullptr;
     q->res_ld = res ? res->ld : 0;
@@ -688,18 +656,8 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
                     int dil) {
     memset(L, 0, sizeof(*L));
     if (cin % 32 != 0 || cin > 1024 || dil < 1 || dil > 8) { set_err("cam_dense: cin must be a multiple of 32 (<= 1024), dilation <= 8"); return false; }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)cin, 128};
-        cuuint64_t str[1] = {(cuuint64_t)cin * 2};
-        cuuint32_t box[2] = {64, 128};
-        if (!encode_map(&L->w1map, dt, W1, 2, dims, str, box, 128)) return false;
-    }
-    {
-        cuuint64_t dims[2] = {384, 32};
-        cuuint64_t str[1] = {384 * 2};
-        cuuint32_t box[2] = {64, 32};
-        if (!encode_map(&L->wlmap, dt, Wl, 2, dims, str, box, 128)) return false;
-    }
+    if (!encode_matrix(&L->w1map, dt, W1, cin, 128, {64, 128}, 128) || !encode_matrix(&L->wlmap, dt, Wl, 3 * 128, 32, {64, 32}, 128))
+        return false;
     L->bn1_scale = bn1_scale; L->bn1_shift = bn1_shift; L->bias2 = bias2;
     L->w1c_t = w1c_t; L->b1c = b1c; L->w2c_t = w2c_t; L->b2c = b2c;
     L->cin = cin; L->dil = dil;
@@ -709,7 +667,7 @@ bool cam_layer_fill(WsCamLayer* L, int dt, const void* W1, const void* Wl, const
 OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std::vector<WsCamLayer>& layers,
                           const std::vector<std::array<const void*, 2>>& weights, int l0, int l1, PlanOp* op, const int* lens) {
     const int T = X.T, B = X.B;
-    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * 2) % 16 != 0)
+    if (X.dt == WS_F32 || X.F != 1 || T < 1 || T > 512 || (X.ld * ws_esize(X.dt)) % 16 != 0)
         return OpBuild::outside;
     auto q = std::make_shared<WsCamParams>();
     memset(q.get(), 0, sizeof(WsCamParams));
@@ -722,11 +680,7 @@ OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std
     q->nstages = nst;
     q->smem_bytes = ws_cam_smem_bytes(q->nmt, nst);
     q->grid = B;
-    cuuint64_t dims[3] = {(cuuint64_t)X.C, (cuuint64_t)T, (cuuint64_t)B};
-    cuuint64_t str[2] = {(cuuint64_t)X.ld * 2, (cuuint64_t)T * X.ld * 2};
-    cuuint32_t boxx[3] = {64, 128, 1}, boxo[3] = {32, 128, 1};
-    if (!encode_map(&q->xmap, X.dt, X.p, 3, dims, str, boxx, 128)) return OpBuild::error;
-    if (!encode_map(&q->omap, X.dt, X.p, 3, dims, str, boxo, 64)) return OpBuild::error;
+    if (!encode_view(&q->xmap, X, {64, 128, 1}, 128) || !encode_view(&q->omap, X, {32, 128, 1}, 64)) return OpBuild::error;
     const CamRec rec{q, X, {layers.begin() + l0, layers.begin() + l1}, {weights.begin() + l0, weights.begin() + l1}};
     *op = plan_op(rec, [](const CamRec& r, cudaStream_t s) { return ws_cam_launch(r.q.get(), s); }, label_of(rec));
     return OpBuild::built;
