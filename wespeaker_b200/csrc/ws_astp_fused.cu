@@ -215,25 +215,18 @@ __global__ void __launch_bounds__(kThreadsA, 1) ws_astp_fused_kernel(const __gri
     }
 }
 
-}  // namespace
-
-extern "C" const char* ws_astp_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    cudaError_t e = cudaFuncSetAttribute(ws_astp_fused_kernel<WS_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemA);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ws_astp_fused_kernel<WS_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemA);
-    if (e != cudaSuccess) { cudaGetLastError(); return cudaGetErrorString(e); }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
+template <int DT>
+const char* astp_go(const WsAstpParams* p, cudaStream_t s) {
+    if (const char* m = ws_smem_opt_in<ws_astp_fused_kernel<DT>>(kSmemA)) return m;
+    ws_astp_fused_kernel<DT><<<p->grid, kThreadsA, kSmemA, s>>>(*p);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-extern "C" int ws_astp_smem(void) { return kSmemA; }
+}  // namespace
 
 extern "C" const char* ws_astp_launch(const WsAstpParams* p, cudaStream_t s) {
-    if (p->dtype == WS_BF16) ws_astp_fused_kernel<WS_BF16><<<p->grid, kThreadsA, kSmemA, s>>>(*p);
-    else if (p->dtype == WS_F16) ws_astp_fused_kernel<WS_F16><<<p->grid, kThreadsA, kSmemA, s>>>(*p);
-    else return "ws_astp_launch: 16-bit activations only";
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    if (p->dtype == WS_BF16) return astp_go<WS_BF16>(p, s);
+    if (p->dtype == WS_F16) return astp_go<WS_F16>(p, s);
+    return "ws_astp_launch: 16-bit activations only";
 }

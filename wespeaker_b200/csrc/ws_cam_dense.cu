@@ -25,7 +25,6 @@ namespace {
 using namespace ws_tcdev;
 
 constexpr int kCamThreads = 384;
-constexpr int kCamMaxSmem = 222 * 1024;
 constexpr int kCamMaxStages = 6;
 constexpr int kStageBytes = 32 * 1024;       // 16 KB activation panel (128 rows x 64 ch) + 16 KB weight k-block (128 x 64)
 constexpr int kHPad = 8;                     // zero rows in front of t = 0 (>= max dilation; multiple of 8 keeps the swizzle phase)
@@ -318,31 +317,28 @@ __global__ void __launch_bounds__(kCamThreads, 1) ws_cam_dense_kernel(const __gr
     }
 }
 
-}  // namespace
+// shared-memory bytes the kernel needs for (nmt tiles, nstages ring stages)
+constexpr int cam_smem(int nmt, int nstages) { return 2 * (16 + 128 * nmt) * 128 + nstages * kStageBytes + kParamFloats * 4 + 2048; }
+static_assert(cam_smem(4, 2) <= kCamMaxSmem, "the longest utterance (4 M tiles) must fit with the shortest ring");
 
-extern "C" const char* ws_cam_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    cudaError_t e = cudaFuncSetAttribute(ws_cam_dense_kernel<WS_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCamMaxSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ws_cam_dense_kernel<WS_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCamMaxSmem);
-    if (e != cudaSuccess) { cudaGetLastError(); return cudaGetErrorString(e); }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
+template <int DT>
+const char* cam_go(const WsCamParams* p, cudaStream_t s) {
+    if (const char* m = ws_smem_opt_in<ws_cam_dense_kernel<DT>>(kCamMaxSmem)) return m;
+    ws_cam_dense_kernel<DT><<<p->grid, kCamThreads, p->smem_bytes, s>>>(*p);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 
-extern "C" int ws_cam_max_smem(void) { return kCamMaxSmem; }
+}  // namespace
 
-// shared-memory bytes the kernel needs for (nmt tiles, nstages ring stages); 0 if the geometry is not supported
+// cam_smem, or 0 if the geometry is not supported
 extern "C" int ws_cam_smem_bytes(int nmt, int nstages) {
     if (nmt < 1 || nmt > 4 || nstages < 2 || nstages > kCamMaxStages) return 0;
-    return 2 * (16 + 128 * nmt) * 128 + nstages * kStageBytes + kParamFloats * 4 + 2048;
+    return cam_smem(nmt, nstages);
 }
 
 extern "C" const char* ws_cam_launch(const WsCamParams* p, cudaStream_t s) {
-    if (p->dtype == WS_BF16) ws_cam_dense_kernel<WS_BF16><<<p->grid, kCamThreads, p->smem_bytes, s>>>(*p);
-    else if (p->dtype == WS_F16) ws_cam_dense_kernel<WS_F16><<<p->grid, kCamThreads, p->smem_bytes, s>>>(*p);
-    else return "cam_dense: 16-bit activations only";
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    if (p->dtype == WS_BF16) return cam_go<WS_BF16>(p, s);
+    if (p->dtype == WS_F16) return cam_go<WS_F16>(p, s);
+    return "cam_dense: 16-bit activations only";
 }

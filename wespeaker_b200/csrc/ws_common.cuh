@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+
 enum WsDType : int { WS_F32 = 0, WS_BF16 = 1, WS_F16 = 2 };
 // RELU20 = Hardtanh(0, 20), the "ReLU" of the Res2Net / ERes2Net families (eres2net.py:43-52); SILU = v * sigmoid(v) (AFF)
 enum WsAct : int { WS_ACT_NONE = 0, WS_ACT_RELU = 1, WS_ACT_TANH = 2, WS_ACT_SIGMOID = 3, WS_ACT_RELU20 = 4, WS_ACT_SILU = 5 };
@@ -406,49 +408,54 @@ struct WsCamParams {
     const int* lens;          // length-masked batch: frames of each utterance (statistics and padding follow them), or null
 };
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) and the SM count are PER DEVICE: init guards are keyed by the current
-// device so that a second engine on another GPU of the same process gets its opt-in too (one bit per device ordinal).
-inline bool ws_dev_needs_init(unsigned long long* mask, int* dev_out) {
+// Dynamic shared memory per CTA that the host geometry code plans within and the kernels are opted in to.
+constexpr int kMaxDynSmem2 = 226 * 1024;   // conv-GEMM (ws_gemm_tc2.cu): ring + staging + per-channel parameters + scratch
+constexpr int kC3MaxSmem = 222 * 1024;     // halo-resident 3x3 conv (ws_conv3x3.cu)
+constexpr int kCamMaxSmem = 222 * 1024;    // fused CAM++ dense layers (ws_cam_dense.cu)
+constexpr int kRes2MaxSmem = 220 * 1024;   // fused Res2 chain (ws_res2_fused.cu)
+
+// Opts one kernel instance into `bytes` of dynamic shared memory on the current device.  The attribute is per device, so
+// each instance keeps one bit per device ordinal, set once the call succeeded (ordinals >= 64 set it on every call).  Two
+// threads may both set it; that is harmless.  On failure the runtime's last error is cleared and its message returned.
+template <auto Kernel>
+inline const char* ws_smem_opt_in(int bytes) {
+    static std::atomic<unsigned long long> done{0};
     int dev = 0;
     cudaGetDevice(&dev);
-    *dev_out = dev;
-    return dev < 0 || dev >= 64 || ((*mask >> dev) & 1ull) == 0;
+    const unsigned long long bit = dev >= 0 && dev < 64 ? 1ull << dev : 0;
+    if (done.load() & bit) return nullptr;
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return cudaGetErrorString(e);
+    }
+    done.fetch_or(bit);
+    return nullptr;
 }
-inline void ws_dev_mark_init(unsigned long long* mask, int dev) {
-    if (dev >= 0 && dev < 64) *mask |= 1ull << dev;
-}
+
 inline int ws_num_sms() {
-    static int sms[64] = {0};
+    static std::atomic<int> sms[64] = {};   // per device ordinal; 0 = not yet queried
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) return 132;
-    if (sms[dev] == 0) {
-        int n = 0;
+    int n = sms[dev].load();
+    if (n == 0) {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        sms[dev] = n > 0 ? n : 132;
+        if (n <= 0) n = 132;
+        sms[dev].store(n);
     }
-    return sms[dev];
+    return n;
 }
 
 #ifdef __cplusplus
 extern "C" {
 #endif
-const char* ws_astp_init(void);
-int ws_astp_smem(void);
 const char* ws_astp_launch(const WsAstpParams* p, cudaStream_t s);
-const char* ws_res2_init(void);
 const char* ws_res2_launch(const WsRes2Params* p, cudaStream_t s);
-const char* ws_cam_init(void);
-int ws_cam_max_smem(void);
 const char* ws_cam_launch(const WsCamParams* p, cudaStream_t s);
-const char* ws_c3_init(void);
-int ws_c3_max_smem(void);
 const char* ws_c3_launch(const WsC3Params* p, cudaStream_t s);
-const char* ws_tc3_init(void);
 int ws_tc3_max_clusters(int cl);   // co-resident clusters of `cl` CTAs on this device (0 = query failed)
 const char* ws_tc3_launch(const WsTc2Params* p, cudaStream_t s);
-const char* ws_tc2_init(void);
-int ws_tc2_max_smem(void);
 const char* ws_tc2_launch(const WsTc2Params* p, cudaStream_t s);
 const char* ws_simt_launch(const WsSimtParams* p, cudaStream_t s);
 #ifdef __cplusplus

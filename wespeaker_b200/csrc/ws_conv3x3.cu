@@ -24,7 +24,6 @@ namespace {
 using namespace ws_tcdev;
 
 constexpr int kC3Threads = 384;
-constexpr int kC3MaxSmem = 222 * 1024;
 
 // Walk over this CTA's contiguous range of output-row steps.  The (f, b group, t tile, n tile) decomposition costs integer
 // divisions only once; every role advances it incrementally (a 64-bit div/mod per step and role was ~5k cycles per step of
@@ -339,55 +338,36 @@ __global__ void __launch_bounds__(kC3Threads, 1) ws_conv3x3_kernel(const __grid_
 
 namespace {
 template <int DT, int ROWB, int NPAN, int NMT, int NN>
-const char* c3_launch_one(const WsC3Params* p, cudaStream_t s, bool attr_only) {
-    if (attr_only) {
-        cudaError_t e = cudaFuncSetAttribute(ws_conv3x3_kernel<DT, ROWB, NPAN, NMT, NN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kC3MaxSmem);
-        return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
-    }
-    ws_conv3x3_kernel<DT, ROWB, NPAN, NMT, NN><<<p->grid, kC3Threads, p->smem_bytes, s>>>(*p);
+const char* c3_launch_one(const WsC3Params* p, cudaStream_t s) {
+    constexpr auto kernel = ws_conv3x3_kernel<DT, ROWB, NPAN, NMT, NN>;
+    if (const char* m = ws_smem_opt_in<kernel>(kC3MaxSmem)) return m;
+    kernel<<<p->grid, kC3Threads, p->smem_bytes, s>>>(*p);
     return nullptr;
 }
 template <int DT, int ROWB, int NPAN, int NMT>
-const char* c3_dispatch_n(const WsC3Params* p, cudaStream_t s, bool attr_only, int n) {
-    if (n == 32) return c3_launch_one<DT, ROWB, NPAN, NMT, 32>(p, s, attr_only);
-    if (n == 64) return c3_launch_one<DT, ROWB, NPAN, NMT, 64>(p, s, attr_only);
-    if (n == 128) return c3_launch_one<DT, ROWB, NPAN, NMT, 128>(p, s, attr_only);
+const char* c3_dispatch_n(const WsC3Params* p, cudaStream_t s, int n) {
+    if (n == 32) return c3_launch_one<DT, ROWB, NPAN, NMT, 32>(p, s);
+    if (n == 64) return c3_launch_one<DT, ROWB, NPAN, NMT, 64>(p, s);
+    if (n == 128) return c3_launch_one<DT, ROWB, NPAN, NMT, 128>(p, s);
     return "conv3x3: unsupported channel tile";
 }
 // (operand row bytes, K panels per tap, M tiles per step, output channels): 64-byte rows only exist with one panel (C = 32)
 template <int DT>
-const char* c3_dispatch(const WsC3Params* p, cudaStream_t s, bool attr_only, int rowb, int npan, int nmt, int n) {
-    if (rowb == 64 && npan == 1 && nmt == 1) return c3_dispatch_n<DT, 64, 1, 1>(p, s, attr_only, n);
-    if (rowb == 64 && npan == 1 && nmt == 2) return c3_dispatch_n<DT, 64, 1, 2>(p, s, attr_only, n);
-    if (rowb == 128 && npan == 1 && nmt == 1) return c3_dispatch_n<DT, 128, 1, 1>(p, s, attr_only, n);
-    if (rowb == 128 && npan == 1 && nmt == 2) return c3_dispatch_n<DT, 128, 1, 2>(p, s, attr_only, n);
-    if (rowb == 128 && npan == 2 && nmt == 1) return c3_dispatch_n<DT, 128, 2, 1>(p, s, attr_only, n);
-    if (rowb == 128 && npan == 2 && nmt == 2) return c3_dispatch_n<DT, 128, 2, 2>(p, s, attr_only, n);
+const char* c3_dispatch(const WsC3Params* p, cudaStream_t s, int rowb, int npan, int nmt, int n) {
+    if (rowb == 64 && npan == 1 && nmt == 1) return c3_dispatch_n<DT, 64, 1, 1>(p, s, n);
+    if (rowb == 64 && npan == 1 && nmt == 2) return c3_dispatch_n<DT, 64, 1, 2>(p, s, n);
+    if (rowb == 128 && npan == 1 && nmt == 1) return c3_dispatch_n<DT, 128, 1, 1>(p, s, n);
+    if (rowb == 128 && npan == 1 && nmt == 2) return c3_dispatch_n<DT, 128, 1, 2>(p, s, n);
+    if (rowb == 128 && npan == 2 && nmt == 1) return c3_dispatch_n<DT, 128, 2, 1>(p, s, n);
+    if (rowb == 128 && npan == 2 && nmt == 2) return c3_dispatch_n<DT, 128, 2, 2>(p, s, n);
     return "conv3x3: unsupported (row bytes, K panels, M tiles) combination";
 }
 }  // namespace
 
-extern "C" const char* ws_c3_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    const int combos[6][3] = {{64, 1, 1}, {64, 1, 2}, {128, 1, 1}, {128, 1, 2}, {128, 2, 1}, {128, 2, 2}};
-    for (auto& c : combos)
-        for (int n : {32, 64, 128}) {
-            const char* m = c3_dispatch<WS_BF16>(nullptr, nullptr, true, c[0], c[1], c[2], n);
-            if (!m) m = c3_dispatch<WS_F16>(nullptr, nullptr, true, c[0], c[1], c[2], n);
-            if (m) { cudaGetLastError(); return m; }
-        }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
-}
-
-extern "C" int ws_c3_max_smem(void) { return kC3MaxSmem; }
-
 extern "C" const char* ws_c3_launch(const WsC3Params* p, cudaStream_t s) {
     const char* m;
-    if (p->dtype == WS_BF16) m = c3_dispatch<WS_BF16>(p, s, false, p->row_bytes, p->npan, p->n_mt, p->N);
-    else if (p->dtype == WS_F16) m = c3_dispatch<WS_F16>(p, s, false, p->row_bytes, p->npan, p->n_mt, p->N);
+    if (p->dtype == WS_BF16) m = c3_dispatch<WS_BF16>(p, s, p->row_bytes, p->npan, p->n_mt, p->N);
+    else if (p->dtype == WS_F16) m = c3_dispatch<WS_F16>(p, s, p->row_bytes, p->npan, p->n_mt, p->N);
     else return "conv3x3: 16-bit activations only";
     if (m) return m;
     cudaError_t e = cudaGetLastError();

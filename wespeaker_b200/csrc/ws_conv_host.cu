@@ -312,7 +312,7 @@ static OpBuild build_tc2(const ConvSpec& s, WsTc2Params* q, int cl = 1) {
     if (!tc2_geometry(s, q)) return OpBuild::error;
     q->nout = (s.split ? 2 : 1) * (q->has_out2 ? 2 : 1);
     const int nstage_bufs = q->nout + (q->has_epin ? 1 : 0);
-    const int budget = ws_tc2_max_smem() - 1024;
+    const int budget = kMaxDynSmem2 - 1024;
     q->epi_generic = s.epi_generic;
     const int mtiles = q->tiles_t * q->tiles_f * q->tiles_b;
     const int g_num_sms = ws_num_sms();
@@ -535,7 +535,7 @@ OpBuild make_conv3x3_op(const View& x, const View& out, const void* W, const flo
     q->npan = Cin / q->kc;
     q->N = Cout; q->n_nt = 1;
     // ---- geometry of one ring slot / one step: first candidate whose ring (>= 4 slots) fits in shared memory
-    const int budget = ws_c3_max_smem();
+    const int budget = kC3MaxSmem;
     auto try_geom = [&](bool case_b, int tb, int n_mt) -> bool {
         q->case_b = case_b ? 1 : 0;
         q->tb = tb; q->n_mt = n_mt;
@@ -675,7 +675,7 @@ OpBuild make_cam_dense_op(const View& X, const WsCamLayer* layers_dev, const std
     q->B = B; q->T = T; q->nmt = (T + 127) / 128; q->seg_len = kCamSegLen; q->dtype = X.dt;
     q->hrows = 16 + 128 * q->nmt;
     int nst = 6;
-    while (nst >= 2 && ws_cam_smem_bytes(q->nmt, nst) > ws_cam_max_smem()) --nst;
+    while (nst >= 2 && ws_cam_smem_bytes(q->nmt, nst) > kCamMaxSmem) --nst;
     if (nst < 2) return OpBuild::outside;
     q->nstages = nst;
     q->smem_bytes = ws_cam_smem_bytes(q->nmt, nst);
@@ -736,7 +736,6 @@ extern "C" int ws_conv(const ws_conv_desc* d, void* stream) {
     s.epi.colsum = d->colsum; s.epi.colsum_T = d->colsum ? To : 0;
     { const char* eg = getenv("WS_EPI_GENERIC"); s.epi_generic = eg != nullptr && atoi(eg) != 0; }
     PlanOp op;
-    if (d->use_tc) { WS_CKS(ws_tc2_init()); WS_CKS(ws_tc3_init()); WS_CKS(ws_c3_init()); WS_CKS(ws_astp_init()); }
     bool done = false;
     if (d->use_tc >= 4 && d->kf == 3 && d->kt == 3 && d->dil_f == 1 && d->dil_t == 1 && d->pad_f == 1 && d->pad_t == 1 &&
         d->stride_f >= 1 && d->stride_f <= 2 && d->stride_t >= 1 && d->stride_t <= 2 && d->scale == nullptr && d->x_lo == nullptr && d->colsum == nullptr &&

@@ -148,15 +148,6 @@ const char* ws_launch_dwconv3x3(const WsDwconv3x3& a, cudaStream_t s) {
         !aligned16(shift) || (out_lo != nullptr && (dt != WS_F32 || !aligned16(out_lo))))
         return "dwconv3x3: C, x_ld and out_ld must be multiples of 8 (16-bit) / 4 (fp32), buffers 16-byte aligned, out_lo fp32 only";
     if (B < 1 || F < 1 || T < 1 || B > 65535) return "dwconv3x3: bad extents";
-    static unsigned long long attr = 0;   // per-device opt-in (ws_common.cuh)
-    int dev = 0;
-    if (ws_dev_needs_init(&attr, &dev)) {
-        cudaError_t e = cudaFuncSetAttribute(dwconv3x3_kernel<WS_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(dwconv3x3_kernel<WS_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(dwconv3x3_kernel<WS_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-        if (e != cudaSuccess) return cudaGetErrorString(e);
-        ws_dev_mark_init(&attr, dev);
-    }
     // balanced bands and tiles: F = 10 is one band of 10 rows, F = 40 four; T = 100 is four tiles of 25 frames
     const int nband = (F + kMaxFB - 1) / kMaxFB, fb = (F + nband - 1) / nband;
     const int ntile = (T + kTT - 1) / kTT, tt = (T + ntile - 1) / ntile;
@@ -164,6 +155,10 @@ const char* ws_launch_dwconv3x3(const WsDwconv3x3& a, cudaStream_t s) {
     if ((long long)nchunk * ntile > 0x7fffffffLL || nband > 65535) return "dwconv3x3: tensor too large";
     const dim3 grid(nchunk * ntile, nband, B);
     const int smem = (fb + 2) * (tt + 2) * kCh * ws_esize(dt);
+    const char* m = dt == WS_BF16  ? ws_smem_opt_in<dwconv3x3_kernel<WS_BF16>>(kMaxSmem)
+                    : dt == WS_F16 ? ws_smem_opt_in<dwconv3x3_kernel<WS_F16>>(kMaxSmem)
+                                   : ws_smem_opt_in<dwconv3x3_kernel<WS_F32>>(kMaxSmem);
+    if (m) return m;
     if (dt == WS_BF16)
         dwconv3x3_kernel<WS_BF16><<<grid, kThreads, smem, s>>>(x, x_ld, a.w, a.shift, out, nullptr, out_ld, F, T, C, fb, tt, nchunk, a.lens);
     else if (dt == WS_F16)

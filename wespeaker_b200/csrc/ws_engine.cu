@@ -311,14 +311,16 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
         return 1;
     }
     WS_CK(cudaSetDevice(device));
+    int cc_major = 0, cc_minor = 0;
+    WS_CK(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
+    WS_CK(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (cc_major != 9 || cc_minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+        set_err("ws_engine_create: device " + std::to_string(device) + " has compute capability " + std::to_string(cc_major) + "." +
+                std::to_string(cc_minor) + "; the kernels are built for sm_90a (compute capability 9.0) only");
+        return 1;
+    }
     std::unique_ptr<ws_engine> e(new ws_engine());
     if (configure_engine(e.get(), model_name, precision, feat_dim, embed_dim, device)) return 1;
-    WS_CKS(ws_tc2_init());
-    WS_CKS(ws_res2_init());
-    WS_CKS(ws_astp_init());
-    WS_CKS(ws_tc3_init());
-    WS_CKS(ws_c3_init());
-    WS_CKS(ws_cam_init());
     WS_CK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
     e->lanes[0] = e->st;
     for (int i = 1; i < ws_engine::kLanes; ++i) WS_CK(cudaStreamCreateWithFlags(&e->lanes[i], cudaStreamNonBlocking));

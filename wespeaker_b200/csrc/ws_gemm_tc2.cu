@@ -32,7 +32,6 @@ namespace {
 using namespace ws_tcdev;
 
 constexpr int kThreads2 = 384;
-constexpr int kMaxDynSmem2 = 226 * 1024;
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -413,25 +412,13 @@ __global__ void __launch_bounds__(kThreads2, 1) ws_conv_gemm_tc2_kernel(const __
 
 namespace {
 template <int KIND, int LEAN, int CL, int BN = 0>
-inline cudaError_t tc2_attr1() {
-    return cudaFuncSetAttribute(ws_conv_gemm_tc2_kernel<KIND, LEAN, CL, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem2);
-}
-template <int CL>
-inline cudaError_t tc2_attr() {
-    cudaError_t e = tc2_attr1<0, 0, CL>();
-    if (e == cudaSuccess) e = tc2_attr1<1, 0, CL>();
-    if (e == cudaSuccess) e = tc2_attr1<0, WS_F32 + 1, CL>();
-    if (e == cudaSuccess) e = tc2_attr1<1, WS_BF16 + 1, CL>();
-    if (e == cudaSuccess) e = tc2_attr1<1, WS_F16 + 1, CL>();
-    if (e == cudaSuccess) e = tc2_attr1<1, WS_BF16 + 1, CL, 256>();
-    if (e == cudaSuccess) e = tc2_attr1<1, WS_F16 + 1, CL, 256>();
-    return e;
-}
-template <int KIND, int LEAN, int CL, int BN = 0>
-inline cudaError_t tc2_go(const WsTc2Params* p, cudaStream_t s) {
+const char* tc2_go(const WsTc2Params* p, cudaStream_t s) {
+    constexpr auto kernel = ws_conv_gemm_tc2_kernel<KIND, LEAN, CL, BN>;
+    if (const char* m = ws_smem_opt_in<kernel>(kMaxDynSmem2)) return m;
+    cudaError_t e;
     if constexpr (CL == 1) {
-        ws_conv_gemm_tc2_kernel<KIND, LEAN, 1, BN><<<p->grid, kThreads2, p->smem_bytes, s>>>(*p);
-        return cudaGetLastError();
+        kernel<<<p->grid, kThreads2, p->smem_bytes, s>>>(*p);
+        e = cudaGetLastError();
     } else {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(kThreads2); cfg.dynamicSmemBytes = (size_t)p->smem_bytes; cfg.stream = s;
@@ -439,11 +426,12 @@ inline cudaError_t tc2_go(const WsTc2Params* p, cudaStream_t s) {
         at.id = cudaLaunchAttributeClusterDimension;
         at.val.clusterDim.x = CL; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
         cfg.attrs = &at; cfg.numAttrs = 1;
-        return cudaLaunchKernelEx(&cfg, ws_conv_gemm_tc2_kernel<KIND, LEAN, CL, BN>, *p);
+        e = cudaLaunchKernelEx(&cfg, kernel, *p);
     }
+    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
 template <int CL>
-inline cudaError_t tc2_dispatch(const WsTc2Params* p, cudaStream_t s, int lean) {
+const char* tc2_dispatch(const WsTc2Params* p, cudaStream_t s, int lean) {
     if (p->bn == 256) return lean == WS_BF16 + 1 ? tc2_go<1, WS_BF16 + 1, CL, 256>(p, s) : tc2_go<1, WS_F16 + 1, CL, 256>(p, s);
     if (lean == WS_F32 + 1) return tc2_go<0, WS_F32 + 1, CL>(p, s);
     if (lean == WS_BF16 + 1) return tc2_go<1, WS_BF16 + 1, CL>(p, s);
@@ -451,55 +439,37 @@ inline cudaError_t tc2_dispatch(const WsTc2Params* p, cudaStream_t s, int lean) 
     if (p->kind == 0) return tc2_go<0, 0, CL>(p, s);
     return tc2_go<1, 0, CL>(p, s);
 }
-}  // namespace
 
-extern "C" const char* ws_tc2_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    cudaError_t e = tc2_attr<1>();
-    if (e != cudaSuccess) { cudaGetLastError(); return cudaGetErrorString(e); }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
-}
-
-extern "C" const char* ws_tc3_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    cudaError_t e = tc2_attr<2>();
-    if (e == cudaSuccess) e = tc2_attr<4>();
-    if (e != cudaSuccess) { cudaGetLastError(); return cudaGetErrorString(e); }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
-}
-
-// ring + staging + per-channel parameters + epilogue scratch, per CTA (the same for the cluster variant)
-extern "C" int ws_tc2_max_smem(void) { return kMaxDynSmem2; }
-
-// how many clusters of `cl` CTAs (at the kernel's maximum shared memory) the device keeps resident at once: GPCs whose SM
-// count is not a multiple of cl leave SMs idle, so this can be below num_sms / cl
-extern "C" int ws_tc3_max_clusters(int cl) {
-    static int cache[64][2];
-    static bool have[64][2];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || (cl != 2 && cl != 4)) return 0;
-    const int k = cl == 4;
-    if (have[dev][k]) return cache[dev][k];
-    if (ws_tc3_init() != nullptr) return 0;
+// how many clusters of CL CTAs (at the kernel's maximum shared memory) the device keeps resident at once: GPCs whose SM
+// count is not a multiple of CL leave SMs idle, so this can be below num_sms / CL
+template <int CL>
+int tc3_query_clusters() {
+    constexpr auto kernel = ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, CL, 0>;
+    if (ws_smem_opt_in<kernel>(kMaxDynSmem2) != nullptr) return 0;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(ws_num_sms() / cl * cl));
+    cfg.gridDim = dim3((unsigned)(ws_num_sms() / CL * CL));
     cfg.blockDim = dim3(kThreads2);
     cfg.dynamicSmemBytes = kMaxDynSmem2;
     cudaLaunchAttribute at;
     at.id = cudaLaunchAttributeClusterDimension;
-    at.val.clusterDim.x = (unsigned)cl; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+    at.val.clusterDim.x = CL; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
     cfg.attrs = &at; cfg.numAttrs = 1;
     int n = 0;
-    cudaError_t e = cl == 4 ? cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 4, 0>, &cfg)
-                            : cudaOccupancyMaxActiveClusters(&n, ws_conv_gemm_tc2_kernel<1, WS_BF16 + 1, 2, 0>, &cfg);
-    if (e != cudaSuccess) { cudaGetLastError(); n = 0; }
-    cache[dev][k] = n; have[dev][k] = true;
+    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return n;
+}
+}  // namespace
+
+extern "C" int ws_tc3_max_clusters(int cl) {
+    static std::atomic<int> cache[64][2] = {};   // per device ordinal and cluster size; 0 = not yet queried
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || (cl != 2 && cl != 4)) return 0;
+    std::atomic<int>& slot = cache[dev][cl == 4];
+    int n = slot.load();
+    if (n == 0) {
+        n = cl == 4 ? tc3_query_clusters<4>() : tc3_query_clusters<2>();
+        slot.store(n);
+    }
     return n;
 }
 
@@ -516,8 +486,7 @@ extern "C" const char* ws_tc2_launch(const WsTc2Params* p, cudaStream_t s) {
     const int lean = p->epi_generic ? 0 : ws_tc_lean_kind(p);
     if (const char* m = ws_tc_colsum_check(p, lean)) return m;
     if (const char* m = ws_tc2_wide_check(p, lean)) return m;
-    const cudaError_t e = tc2_dispatch<1>(p, s, lean);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return tc2_dispatch<1>(p, s, lean);
 }
 
 extern "C" const char* ws_tc3_launch(const WsTc2Params* p, cudaStream_t s) {
@@ -525,6 +494,5 @@ extern "C" const char* ws_tc3_launch(const WsTc2Params* p, cudaStream_t s) {
     if (const char* m = ws_tc_colsum_check(p, lean)) return m;
     if (const char* m = ws_tc2_wide_check(p, lean)) return m;
     if (p->cl != 2 && p->cl != 4) return "ws_tc3_launch: cluster size must be 2 or 4";
-    const cudaError_t e = p->cl == 4 ? tc2_dispatch<4>(p, s, lean) : tc2_dispatch<2>(p, s, lean);
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    return p->cl == 4 ? tc2_dispatch<4>(p, s, lean) : tc2_dispatch<2>(p, s, lean);
 }

@@ -1057,15 +1057,10 @@ const char* ws_launch_se_gate(const WsSeGate& a, cudaStream_t s) {
     const int C = x.C, H = a.H;
     if (H != 128 || (C != 512 && C != 1024 && C != 2048 && C != 256)) return "se_gate: expected H=128 and C in {256,512,1024,2048}";
     const size_t smem = (size_t)(2 * C + 8192 + 2 * H) * sizeof(float);
-    static unsigned long long attr = 0;   // per-device opt-in (ws_common.cuh)
-    int dev = 0;
-    if (ws_dev_needs_init(&attr, &dev)) {
-        cudaFuncSetAttribute(se_gate_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        ws_dev_mark_init(&attr, dev);
-    }
     if (smem > 96 * 1024) return "se_gate: channel count too large for shared memory";
     if (a.colsum != nullptr && x.T < 128) return "se_gate: fused column sums need >= 128 frames per utterance";
     if (a.lens != nullptr && a.colsum != nullptr) return "se_gate: fused column sums are not available for length-masked batches";
+    if (const char* m = ws_smem_opt_in<se_gate_kernel<128>>(96 * 1024)) return m;
     se_gate_kernel<128><<<(x.B + 1) / 2, 512, smem, s>>>(x.p, x.dt, x.B, x.T, C, x.ld, a.W1, a.b1, a.W2t, a.b2, a.gate, a.colsum, a.lens);
     return last_err();
 }

@@ -309,16 +309,11 @@ const char* ws_launch_dgemm_nt(const double* A, const double* Bm, const double* 
     // fp64 tensor path (mma.sync m8n8k4) whenever K is a multiple of the 16-deep k chunk and the operand rows are 16-byte
     // aligned; WS_PLDA_SIMT=1 keeps the FFMA-style kernel as a cross-check
     if (K % DBK == 0 && K >= DBK && ((uintptr_t)A & 15) == 0 && ((uintptr_t)Bm & 15) == 0 && getenv("WS_PLDA_SIMT") == nullptr) {
-        static unsigned long long attr = 0;
-        int dev = 0;
-        if (ws_dev_needs_init(&attr, &dev)) {
-            cudaFuncSetAttribute(dgemm_nt_dmma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDmmaSmem);
-            cudaFuncSetAttribute(dgemm_nt_dmma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDmmaSmem);
-            ws_dev_mark_init(&attr, dev);
-        }
         const long long dy = (M + DBM - 1) / DBM, dx = (N + DBN - 1) / DBN;
         if (dy > 65535) return "dgemm_nt: M too large for one launch (tile the enroll rows)";
         dim3 dgrid((unsigned)dx, (unsigned)dy);
+        if (const char* m = out_is_f64 ? ws_smem_opt_in<dgemm_nt_dmma_kernel<1>>(kDmmaSmem) : ws_smem_opt_in<dgemm_nt_dmma_kernel<0>>(kDmmaSmem))
+            return m;
         if (out_is_f64) dgemm_nt_dmma_kernel<1><<<dgrid, 256, kDmmaSmem, s>>>(A, Bm, rowc, colc, out, M, N, K, out_ld);
         else dgemm_nt_dmma_kernel<0><<<dgrid, 256, kDmmaSmem, s>>>(A, Bm, rowc, colc, out, M, N, K, out_ld);
         return last_err();

@@ -215,32 +215,20 @@ __global__ void __launch_bounds__(384, 1) ws_res2_fused_kernel(const __grid_cons
     }
 }
 
-}  // namespace
-
-extern "C" const char* ws_res2_init(void) {
-    static unsigned long long done = 0;
-    int dev = 0;
-    if (!ws_dev_needs_init(&done, &dev)) return nullptr;
-    cudaError_t e = cudaFuncSetAttribute(ws_res2_fused_kernel<WS_BF16, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ws_res2_fused_kernel<WS_F16, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ws_res2_fused_kernel<WS_BF16, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(ws_res2_fused_kernel<WS_F16, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-    if (e != cudaSuccess) { cudaGetLastError(); return cudaGetErrorString(e); }
-    ws_dev_mark_init(&done, dev);
-    return nullptr;
+template <int DT, int W8>
+const char* res2_go(const WsRes2Params* p, cudaStream_t s) {
+    constexpr auto kernel = ws_res2_fused_kernel<DT, W8>;
+    if (const char* m = ws_smem_opt_in<kernel>(kRes2MaxSmem)) return m;
+    kernel<<<p->grid, 384, p->smem_bytes, s>>>(*p);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
 }
+
+}  // namespace
 
 extern "C" const char* ws_res2_launch(const WsRes2Params* p, cudaStream_t s) {
     if (p->dtype != WS_BF16 && p->dtype != WS_F16) return "res2_fused: 16-bit activations only";
-    if (p->w8 == 128) {
-        if (p->dtype == WS_BF16) ws_res2_fused_kernel<WS_BF16, 128><<<p->grid, 384, p->smem_bytes, s>>>(*p);
-        else ws_res2_fused_kernel<WS_F16, 128><<<p->grid, 384, p->smem_bytes, s>>>(*p);
-    } else if (p->w8 == 64) {
-        if (p->dtype == WS_BF16) ws_res2_fused_kernel<WS_BF16, 64><<<p->grid, 384, p->smem_bytes, s>>>(*p);
-        else ws_res2_fused_kernel<WS_F16, 64><<<p->grid, 384, p->smem_bytes, s>>>(*p);
-    } else {
-        return "res2_fused: groups of 64 or 128 channels only";
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+    if (p->w8 != 64 && p->w8 != 128) return "res2_fused: groups of 64 or 128 channels only";
+    if (p->w8 == 128) return p->dtype == WS_BF16 ? res2_go<WS_BF16, 128>(p, s) : res2_go<WS_F16, 128>(p, s);
+    return p->dtype == WS_BF16 ? res2_go<WS_BF16, 64>(p, s) : res2_go<WS_F16, 64>(p, s);
 }
