@@ -39,12 +39,25 @@ int ws_engine_create(const char* model_name, const char* precision, int feat_dim
  * against the plan builder (missing keys, shapes, kernel envelopes) on a host without a GPU.  Every compute entry point
  * returns an error on such an engine. */
 int ws_engine_create_plan_check(const char* model_name, const char* precision, int feat_dim, int embed_dim, ws_engine** out);
-/* options: "two_emb_layer", "emb_bn" (model_args), "cuda_graph" (default 1),
- * "sample_rate" (8000 or 16000, default 16000: the rate of the waveforms the extract_wav entry points receive; their fbank
- * writes feat_dim mel bins, 4 <= feat_dim <= 128; any other rate is refused - resample first, as the reference does),
- * "tc_version" (2: persistent / TMA-store tensor-core kernel, 3 (default): + weight-sharing CTA clusters on the large layers;
- * any other value is an error),
- * "res2_fused" (default 1: ECAPA Res2 chains run as one fused persistent kernel per stage for 16-bit precisions) */
+/* Engine options, "name" (default): what the option selects.  A flag takes any value, nonzero meaning on; an unknown name
+ * or a value outside the listed ones is an error.  Setting any option but sample_rate drops the engine's cached plans.
+ *   "two_emb_layer" (0)  model_args of ResNet, Res2Net / ERes2Net and Gemini DF-ResNet: two segment layers, not one
+ *   "emb_bn" (0)         model_args of ECAPA-TDNN: the BatchNorm bn2 after the embedding layer
+ *   "cuda_graph" (1)     replay each plan as one CUDA graph; 0 launches its kernels one by one
+ *   "res2_fused" (1)     16-bit precisions: each ECAPA Res2 chain runs as one fused persistent kernel
+ *   "se_fused" (1)       ECAPA with 512 or 1024 channels: each SE block's squeeze and gate run as one kernel
+ *   "se_colsum" (1)      with se_fused, 16-bit precisions, T >= 128, no length mask: the SE squeeze reads column sums the
+ *                        preceding conv's epilogue wrote
+ *   "conv3x3" (1)        16-bit precisions: 3x3 pad-1 convs run on the halo-resident kernel where the shape fits
+ *   "cam_fused" (1)      16-bit precisions, T <= 1024: CAM++ dense layers run on the fused kernel (length-masked CAM++
+ *                        plans need it)
+ *   "cam_block" (1)      with cam_fused: one launch per CAM++ dense block; 0: one per layer
+ *   "astp_fused" (1)     16-bit precisions: attentive statistics pooling (linear2, softmax, statistics) runs as one kernel
+ *   "plan_trace" (0)     real engines: ws_engine_plan_trace may write the plan with device addresses
+ *   "tc_version" (3)     2: persistent / TMA-store tensor-core kernel; 3: + weight-sharing CTA clusters on the large layers.
+ *                        fp32 runs FFMA whatever it says
+ *   "sample_rate" (16000) 8000 or 16000: the rate of the waveforms the extract_wav entry points receive; their fbank writes
+ *                        feat_dim mel bins, 4 <= feat_dim <= 128 (resample other rates first, as the reference does) */
 int ws_engine_set_option(ws_engine* e, const char* key, long long value);
 /* one reference state_dict entry (fp32 host data, reference key names, SURVEY.md Appendix C). */
 int ws_engine_set_tensor(ws_engine* e, const char* key, const float* host_data, const long long* shape, int ndim);

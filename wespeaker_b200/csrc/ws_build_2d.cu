@@ -18,7 +18,7 @@ View basic_block(Builder& b, const std::string& p, const View& x, int cout, int 
     const View h = hbuf.shaped(x.B, Fo, To, cout), o = obuf.shaped(x.B, Fo, To, cout);
     if (!b.conv3x3(x, h, b.w.act("w:" + p + ".conv1", w1), b.w.f32("bnh:" + p + ".bn1", h1), WS_ACT_RELU, sf, st_, lvl)) return none;
     const bool has_sc = b.e.sd.count(p + ".shortcut.0.weight") != 0;
-    if (b.halo3x3() && (cout == 32 || cout == 64 || cout == 128)) {
+    if (b.fused(b.e.opts.conv3x3) && (cout == 32 || cout == 64 || cout == 128)) {
         // conv2 on the halo-resident kernel: the 1x1 strided shortcut conv (+ its BN) is written to `o` first and then
         // read back as the residual, in place (each output element is read and written by the same CTA step).  conv2's op is
         // built first: if the shape is outside the kernel's envelope nothing has been emitted yet.  (The channel counts the
@@ -178,7 +178,7 @@ bool build_resnet(Builder& b) {
         }
     }
     if (!b.good()) return false;
-    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0);
+    return resnet_tail(b, cur, e.opts.two_emb_layer);
 }
 
 // ----------------------------------------------------------------------------------------------- Res2Net / ERes2Net
@@ -438,7 +438,7 @@ bool build_res2net(Builder& b) {
         cur = f;
     }
     if (!b.good()) return false;
-    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0);
+    return resnet_tail(b, cur, e.opts.two_emb_layer);
 }
 
 // ----------------------------------------------------------------------------------------------- SimAM-ResNet + ASP
@@ -671,7 +671,7 @@ bool build_gemini(Builder& b) {
             cur = nx;
         }
     }
-    return resnet_tail(b, cur, e.opt("two_emb_layer", 0) != 0, 1);
+    return resnet_tail(b, cur, e.opts.two_emb_layer, 1);
 }
 
 }  // namespace ws

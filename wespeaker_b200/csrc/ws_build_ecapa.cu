@@ -35,8 +35,8 @@ bool build_ecapa(Builder& b) {
     conv_relu_bn("layer1", x0, out1, 5, 1, 2);
     View xin = out1;
     float* se_colsum = nullptr;
-    if (e.use_tc >= 2 && e.act_dt != WS_F32 && !e.split && T >= 128 && (C == 512 || C == 1024) && e.opt("se_fused", 1) &&
-        e.opt("se_colsum", 1) && !b.p.masked)   // (column sums would include padding rows)
+    if (b.fused(e.opts.se_fused && e.opts.se_colsum) && T >= 128 && (C == 512 || C == 1024) &&
+        !b.p.masked)   // (column sums would include padding rows)
         se_colsum = b.f32((size_t)2 * (((size_t)B * T + 63) / 64) * C);
     for (int L = 2; L <= 4 && b.good(); ++L) {
         const int d = L;
@@ -45,7 +45,7 @@ bool build_ecapa(Builder& b) {
         b.zero_tail(tA, 0);   // (masked plans) the dilated Res2 convs read tA across time
         // Res2Conv1dReluBn (ecapa_tdnn.py:29-78): 7 dependent dilated k=3 convs on w8-channel groups
         bool fused = false;
-        if (e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("res2_fused", 1)) {
+        if (b.fused(e.opts.res2_fused)) {
             // one persistent launch per stage: the chain stays in shared memory / registers (ws_res2_fused.cu)
             std::vector<float> w7((size_t)7 * w8 * 3 * w8), b7((size_t)7 * w8), s7((size_t)7 * w8), h7((size_t)7 * w8);
             bool okw = true;
@@ -115,7 +115,7 @@ bool build_ecapa(Builder& b) {
             b.conv(cs);
         }
         // SE_Connect (ecapa_tdnn.py:113-126) + residual (:157)
-        if (e.opt("se_fused", 1) && (C == 512 || C == 1024)) {
+        if (e.opts.se_fused && (C == 512 || C == 1024)) {
             const int H = 128;   // SE bottleneck width
             const HostT* w2 = b.w.get(pf + ".3.linear2.weight");   // (C, H) -> transposed (H, C) for coalesced reads
             if (!w2) break;
@@ -191,7 +191,7 @@ bool build_ecapa(Builder& b) {
         if ((int)lw->shape[0] != E) { set_err("linear.weight: embed_dim mismatch"); return false; }
         std::vector<float> wf((size_t)E * 3072), bf(E);
         std::vector<float> s2(E, 1.f), h2(E, 0.f);
-        if (e.opt("emb_bn", 0) && !b.w.bn("bn2", true, s2, h2)) return false;
+        if (e.opts.emb_bn && !b.w.bn("bn2", true, s2, h2)) return false;
         for (int o = 0; o < E; ++o) {
             double acc = lb->v[o];
             for (int i = 0; i < 3072; ++i) {

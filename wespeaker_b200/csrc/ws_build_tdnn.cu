@@ -127,7 +127,7 @@ bool build_campplus(Builder& b) {
         b.conv(cs);
     }
     // Fused dense layers (ws_cam_dense.cu): one launch per CAMDenseTDNNLayer (or per block with cam_block = 1) instead of four
-    const bool cam_fused = e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("cam_fused", 1) != 0 && Tp <= 512;
+    const bool cam_fused = b.fused(e.opts.cam_fused) && Tp <= 512;
     for (int bl = 0; bl < 3 && b.good(); ++bl) {
         bool fused_done = false;
         if (cam_fused) {
@@ -163,7 +163,7 @@ bool build_campplus(Builder& b) {
             if (!okl || !b.good()) { b.ok = false; break; }
             const WsCamLayer* ldev = (const WsCamLayer*)b.w.upload("camlayers:" + std::to_string(bl), hl.data(), hl.size() * sizeof(WsCamLayer));
             if (!b.good()) break;
-            const bool whole = e.opt("cam_block", 1) != 0;
+            const bool whole = e.opts.cam_block;
             fused_done = true;
             for (int j = 0; j < nl[bl]; j += whole ? nl[bl] : 1) {
                 const int j1 = whole ? nl[bl] : j + 1;

@@ -52,6 +52,33 @@ const ModelRow kModels[] = {
     {"Gemini_DF_ResNet237", build_gemini, blocks(3, 8, 63, 3)},
 };
 
+// every precision the engine accepts: activation dtype, tensor-core level (ws_engine::tc) and 3xTF32 error compensation
+struct PrecisionRow { const char* name; int act_dt; int tc; bool split; };
+const PrecisionRow kPrecisions[] = {
+    {"fp32", WS_F32, 0, false},
+    {"tf32", WS_F32, 3, false},
+    {"tf32x3", WS_F32, 3, true},
+    {"bf16", WS_BF16, 3, false},
+    {"fp16", WS_F16, 3, false},
+};
+
+// every option ws_engine_set_option accepts, with the field it sets: a flag, or a number it checks first
+struct OptionRow { const char* name; bool EngineOptions::*flag; int EngineOptions::*number; };
+using O = EngineOptions;
+const OptionRow kOptions[] = {
+    {"two_emb_layer", &O::two_emb_layer}, {"emb_bn", &O::emb_bn}, {"cuda_graph", &O::cuda_graph}, {"plan_trace", &O::plan_trace},
+    {"res2_fused", &O::res2_fused}, {"se_fused", &O::se_fused}, {"se_colsum", &O::se_colsum}, {"conv3x3", &O::conv3x3},
+    {"cam_fused", &O::cam_fused}, {"cam_block", &O::cam_block}, {"astp_fused", &O::astp_fused},
+    {"tc_version", nullptr, &O::tc_version}, {"sample_rate", nullptr, &O::sample_rate},
+};
+
+// the row of `table` named `name` (nullptr: none)
+template <class Row, size_t N> const Row* row_named(const Row (&table)[N], const std::string& name) {
+    for (const Row& r : table)
+        if (name == r.name) return &r;
+    return nullptr;
+}
+
 // ------------------------------------------------------------------------------------------------ plan cache
 Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
     auto key = std::make_pair(B, 2 * T + (masked ? 1 : 0));
@@ -95,7 +122,7 @@ Plan* get_plan(ws_engine* e, int B, int T, bool masked = false) {
 
 // staged: kernels the entry point launched ahead of the plan (fbank, CMN, frame counts), counted in last_launches
 int run_plan(ws_engine* e, Plan* p, cudaStream_t s, int staged) {
-    const bool want_graph = e->opt("cuda_graph", 1) != 0 && !p->graph_failed;
+    const bool want_graph = e->opts.cuda_graph && !p->graph_failed;
     if (want_graph && p->gexec == nullptr) {
         cudaGraph_t g = nullptr;
         if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -249,12 +276,12 @@ int begin_run(Run& r, int B, int T, bool masked, int samples = -1, const char* w
     if (const char* nr = not_runnable(e)) { set_err(std::string(r.who) + nr); return 1; }
     if (samples >= 0) {
         // the fbank frontend writes feat_dim mel bins at the engine's sample rate
-        if (const char* why = fbank_unsupported(e->sample_rate, e->feat_dim)) { set_err(std::string(r.who) + ": " + why); return 1; }
-        T = ws_fbank_num_frames_at(samples, e->sample_rate);
+        if (const char* why = fbank_unsupported(e->opts.sample_rate, e->feat_dim)) { set_err(std::string(r.who) + ": " + why); return 1; }
+        T = ws_fbank_num_frames_at(samples, e->opts.sample_rate);
         if (T <= 0) { set_err(std::string(r.who) + ": waveforms shorter than one 25 ms frame"); return 1; }
     }
     if ((r.p = plan_of(e, B, T, masked)) == nullptr) return 1;
-    if (samples >= 0 && (r.fb = fbank_tables(e, window_type, e->sample_rate, e->feat_dim)) == nullptr) return 1;
+    if (samples >= 0 && (r.fb = fbank_tables(e, window_type, e->opts.sample_rate, e->feat_dim)) == nullptr) return 1;
     r.s = r.host || !e->lanes[r.p->lane] ? e->st : e->lanes[r.p->lane];
     if (!r.host) {
         WS_CK(cudaEventRecord(e->ev_in, r.user));
@@ -284,19 +311,13 @@ extern "C" {
 // model name + precision -> engine configuration (shared by ws_engine_create and ws_engine_create_plan_check)
 static int configure_engine(ws_engine* e, const char* model_name, const char* precision, int feat_dim, int embed_dim, int device) {
     e->model = model_name; e->prec = precision; e->feat_dim = feat_dim; e->embed_dim = embed_dim; e->device = device;
-    const ModelRow* row = nullptr;
-    for (const ModelRow& r : kModels)
-        if (e->model == r.name) row = &r;
+    const ModelRow* row = row_named(kModels, e->model);
     if (row == nullptr) { set_err("unknown / out-of-scope model name: " + e->model); return 1; }
     e->build = row->build;
     e->cfg = row->cfg;
-    const std::string p = e->prec;
-    if (p == "fp32") { e->act_dt = WS_F32; e->use_tc = 0; }
-    else if (p == "tf32") { e->act_dt = WS_F32; e->use_tc = 3; }
-    else if (p == "tf32x3") { e->act_dt = WS_F32; e->use_tc = 3; e->split = true; }
-    else if (p == "bf16") { e->act_dt = WS_BF16; e->use_tc = 3; }
-    else if (p == "fp16") { e->act_dt = WS_F16; e->use_tc = 3; }
-    else { set_err("unknown precision (fp32|tf32x3|tf32|bf16|fp16): " + p); return 1; }
+    const PrecisionRow* prec = row_named(kPrecisions, e->prec);
+    if (prec == nullptr) { set_err("unknown precision (fp32|tf32x3|tf32|bf16|fp16): " + e->prec); return 1; }
+    e->act_dt = prec->act_dt; e->tc = prec->tc; e->split = prec->split;
     if (feat_dim % 8 != 0) { set_err("feat_dim must be a multiple of 8"); return 1; }
     return 0;
 }
@@ -345,23 +366,18 @@ int ws_engine_create_plan_check(const char* model_name, const char* precision, i
 
 int ws_engine_set_option(ws_engine* e, const char* key, long long value) {
     if (!e || !key) { set_err("ws_engine_set_option: null argument"); return 1; }
-    const std::string k = key;
-    if (k == "tc_version") {
-        if (value != 2 && value != 3) {
-            set_err("tc_version must be 2 (persistent tensor-core kernel) or 3 (+ weight-sharing clusters); 1, the one-tile-per-CTA "
-                    "kernel, was removed");
-            return 1;
-        }
-        if (e->use_tc) e->use_tc = (int)value;
+    const OptionRow* row = row_named(kOptions, key);
+    if (row == nullptr) { set_err(std::string("unknown option ") + key); return 1; }
+    const bool rate = row->number == &O::sample_rate;
+    if (row->number == &O::tc_version && value != 2 && value != 3) {
+        set_err("tc_version must be 2 (persistent tensor-core kernel) or 3 (+ weight-sharing clusters); 1, the one-tile-per-CTA "
+                "kernel, was removed");
+        return 1;
     }
-    else if (k == "sample_rate") {   // the waveform entry points' rate; plans do not depend on it, so they are kept
-        if (ws_fbank_frame_len((int)value) == 0 || value != (int)value) { set_err("sample_rate must be 8000 or 16000 (resample first)"); return 1; }
-        e->sample_rate = (int)value;
-        return 0;
-    }
-    else if (k != "two_emb_layer" && k != "emb_bn" && k != "cuda_graph" && k != "res2_fused" && k != "se_fused" && k != "se_colsum" && k != "conv3x3" && k != "cam_fused" && k != "cam_block" && k != "astp_fused" && k != "plan_trace") { set_err("unknown option " + k); return 1; }
-    e->opts[k] = value;
-    e->plans.clear();
+    if (rate && (ws_fbank_frame_len((int)value) == 0 || value != (int)value)) { set_err("sample_rate must be 8000 or 16000 (resample first)"); return 1; }
+    if (row->flag) e->opts.*row->flag = value != 0;
+    else e->opts.*row->number = (int)value;
+    if (!rate) e->plans.clear();   // plans do not depend on the waveform entry points' rate, so they are kept
     return 0;
 }
 
@@ -437,8 +453,8 @@ static int extract_wav_masked_impl(ws_engine* e, const void* wav_dev, int wav_is
     if (!e || !wav_dev || !n_samples_dev || !embs_dev || (ragged && !offsets_dev)) { set_err(std::string(who) + ": null argument"); return 1; }
     Run r{e, who, false, (cudaStream_t)stream};
     if (begin_run(r, B, 0, true, max_samples, window_type)) return 1;
-    WS_CKS(ws_launch_frames_from_samples(n_samples_dev, r.p->lens, B, r.p->T, ws_fbank_frame_len(e->sample_rate),
-                                         ws_fbank_frame_shift(e->sample_rate), r.s));
+    WS_CKS(ws_launch_frames_from_samples(n_samples_dev, r.p->lens, B, r.p->T, ws_fbank_frame_len(e->opts.sample_rate),
+                                         ws_fbank_frame_shift(e->opts.sample_rate), r.s));
     if (fbank_into(r.fb, wav_dev, wav_is_i16, wav_ld, max_samples, B, 1, r.p->feats_in, r.s, offsets_dev, r.p->lens)) return 1;
     return finish_run(r, 3, embs_dev, join);
 }
@@ -700,7 +716,7 @@ const char* ws_engine_plan_op_name(ws_engine* e, int B, int T, int i, double* fl
 // holds [address, float offset into the blob area, float count].
 int ws_engine_plan_trace(ws_engine* e, int B, int T, int masked, const char* path) {
     if (!e || !path) { set_err("ws_engine_plan_trace: null argument"); return 1; }
-    if (!e->finalized || (!e->plan_check && e->opt("plan_trace", 0) == 0)) {
+    if (!e->finalized || (!e->plan_check && !e->opts.plan_trace)) {
         set_err("ws_engine_plan_trace: needs a finalized plan-check engine, or a finalized engine with the option plan_trace = 1");
         return 1;
     }

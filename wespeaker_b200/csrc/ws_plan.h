@@ -74,16 +74,27 @@ struct ModelCfg {
     bool fuse = false;
 };
 
+// The engine options at their defaults (ws_engine_set_option; include/wespeaker_b200.h documents each)
+struct EngineOptions {
+    bool two_emb_layer = false, emb_bn = false;   // model_args
+    bool cuda_graph = true, plan_trace = false;
+    // the fused kernels the plan builders may take
+    bool res2_fused = true, se_fused = true, se_colsum = true, conv3x3 = true, cam_fused = true, cam_block = true, astp_fused = true;
+    int tc_version = 3, sample_rate = 16000;   // sample_rate: the waveform entry points' rate (the mel bin count is feat_dim)
+};
+
 }  // namespace ws
 
 struct ws_engine {
     std::string model, prec;
     int feat_dim = 80, embed_dim = 0, device = 0;
     int act_dt = WS_F32;
-    int use_tc = 0;  // 0 FFMA, 2 persistent tensor-core kernel, 3 the same + weight-sharing clusters on large layers (default)
+    int tc = 0;          // the precision's tensor-core level: 0 FFMA, 3 tensor cores
     bool split = false;  // 3xTF32: fp32 activations/weights carry lo twins, GEMMs run 3 error-compensated passes
+    ws::EngineOptions opts;
+    // the level plans use (2 persistent tensor-core kernel, 3 + weight-sharing clusters): fp32 stays on FFMA
+    int use_tc() const { return std::min(tc, opts.tc_version); }
     std::map<const void*, const void*> wlo;  // packed weight -> its lo twin
-    std::map<std::string, long long> opts;
     std::map<std::string, ws::HostT> sd;
     bool finalized = false;
     bool plan_check = false;   // ws_engine_create_plan_check: builds launch plans without a device, never computes
@@ -108,7 +119,6 @@ struct ws_engine {
     int next_lane = 0;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
     std::map<std::tuple<std::string, int, int>, ws::FbankTables> fb;   // key: (window type, sample rate, mel bins)
-    int sample_rate = 16000;   // waveform entry points (option "sample_rate"); the mel bin count is feat_dim
     void* wav_dev = nullptr;
     size_t wav_bytes = 0;
     // double-buffered host->device pipeline (ws_engine_submit_wav_host / ws_engine_collect)
@@ -139,10 +149,6 @@ struct ws_engine {
         for (int i = 1; i < kLanes; ++i)
             if (lanes[i]) cudaStreamDestroy(lanes[i]);
         if (st) cudaStreamDestroy(st);
-    }
-    long long opt(const char* k, long long dflt) const {
-        auto it = opts.find(k);
-        return it == opts.end() ? dflt : it->second;
     }
 };
 
@@ -266,6 +272,8 @@ struct Builder {
     bool ok = true;
     Builder(ws_engine& eng, Plan& pl) : e(eng), p(pl), w(eng) {}
     bool good() const { return ok && w.ok; }
+    // may a fused 16-bit tensor-core kernel build an op: the precision runs those kernels and the option selecting it is on
+    bool fused(bool option) const { return e.use_tc() >= 2 && e.act_dt != WS_F32 && option; }
 
     void* raw(size_t bytes) {
         void* d = nullptr;
@@ -323,7 +331,7 @@ struct Builder {
             s.split = true;
         }
         PlanOp op;
-        if (!make_conv_op(s, e.use_tc, &op)) { ok = false; return; }
+        if (!make_conv_op(s, e.use_tc(), &op)) { ok = false; return; }
         push(std::move(op));
     }
     static WsSrc src_of(const View& v) {
@@ -368,13 +376,11 @@ struct Builder {
         push(WsConvert{p.feats_in, x0.p, (float*)x0.plo, x0.dt, x0.npos() * x0.C}, ws_launch_convert, "convert");
     }
     // The halo-resident 3x3 pad-1 conv (ws_conv3x3.cu: every input row crosses L2 -> SM once instead of once per tap),
-    // out = act(conv(x, W) + bias [+ res]).  halo3x3: whether the precision and the options let convs use it.  halo_conv3x3
-    // returns 1 with *op built (not pushed), 0 when the caller runs the conv-GEMM instead (also when the shape is outside
-    // the kernel's envelope), -1 on error.  lvl: stride level of `out`.
-    bool halo3x3() const { return e.use_tc >= 2 && e.act_dt != WS_F32 && e.opt("conv3x3", 1) != 0; }
+    // out = act(conv(x, W) + bias [+ res]).  halo_conv3x3 returns 1 with *op built (not pushed), 0 when the caller runs the
+    // conv-GEMM instead (also when the shape is outside the kernel's envelope), -1 on error.  lvl: stride level of `out`.
     int halo_conv3x3(const View& x, const View& out, const void* W, const float* bias, const View* res, int act, int sf, int st, int lvl,
                      PlanOp* op) {
-        if (!halo3x3()) return 0;
+        if (!fused(e.opts.conv3x3)) return 0;
         const OpBuild r = make_conv3x3_op(x, out, W, bias, res, act == WS_ACT_RELU20 ? 2 : act == WS_ACT_RELU ? 1 : 0, op, sf, st, lens(lvl));
         if (r == OpBuild::error) ok = false;
         return r == OpBuild::built ? 1 : r == OpBuild::outside ? 0 : -1;
@@ -420,7 +426,7 @@ struct Builder {
     // astp_stats.  lvl: stride level of x
     bool astp_tail(const View& x, const View& h, const void* W2, const float* bias2, float* stats, double eps, int lvl) {
         const int* l = lens(lvl);
-        if (e.use_tc >= 2 && e.opt("astp_fused", 1) && good()) {
+        if (fused(e.opts.astp_fused) && good()) {
             PlanOp op;
             const OpBuild r = make_astp_op(x, h, W2, stats, (float)eps, &op, l);
             if (r == OpBuild::built) { push(std::move(op)); return true; }

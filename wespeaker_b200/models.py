@@ -110,6 +110,13 @@ class B200SpeakerModel(torch.nn.Module):
         self.options[key] = int(value)
         self._drop_engine()
 
+    def engine_options(self) -> dict:
+        """The engine options of this model, in the order the engine receives them: the model_args flags two_emb_layer and
+        emb_bn, then every set_option call (a later value wins)."""
+        opts = {k: 1 for k in ("two_emb_layer", "emb_bn") if self.model_args.get(k)}
+        opts.update(self.options)
+        return opts
+
     # ------------------------------------------------------------------ engine
     def _drop_engine(self):
         if self._engine is not None:
@@ -142,10 +149,7 @@ class B200SpeakerModel(torch.nn.Module):
 
     def _configure(self, L, h):
         """options + reference state_dict -> engine handle, then finalize (packs / folds / converts the weights)."""
-        for opt in ("two_emb_layer", "emb_bn"):
-            if self.model_args.get(opt):
-                _lib.check(L.ws_engine_set_option(h, opt.encode(), 1), "ws_engine_set_option")
-        for k, v in self.options.items():
+        for k, v in self.engine_options().items():
             _lib.check(L.ws_engine_set_option(h, k.encode(), v), "ws_engine_set_option")
         for k, v in self._sd.items():
             if k.endswith("num_batches_tracked"):
@@ -534,10 +538,7 @@ class B200SpeakerModel(torch.nn.Module):
         def wstr(f, t: str):
             b = t.encode()
             f.write(struct.pack("<I", len(b)) + b)
-        opts = {k: int(v) for k, v in self.options.items()}
-        for opt in ("two_emb_layer", "emb_bn"):
-            if self.model_args.get(opt):
-                opts[opt] = 1
+        opts = self.engine_options()
         tensors = [(k, v) for k, v in self._sd.items() if not k.endswith("num_batches_tracked")]
         with open(path, "wb") as f:
             f.write(b"WSPKB200" + struct.pack("<I", 1))
